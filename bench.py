@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py -- pod-fit decisions/s of the autoscaler tick on B200 (driver contract, see DESIGN.md section 6).
+"""bench.py -- pod-fit decisions/s of the autoscaler tick on H100 (see DESIGN.md section 6).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c3|small]
+                    [--dump-outputs DIR]
 
 A "step" is one whole tick of the hot path over one synthetic snapshot (SURVEY.md section 8d):
     occupancy (K1) + get_pods_to_schedule (K0) + get_pending_pods (first-fit pipeline over nodes)
@@ -11,7 +12,10 @@ A "step" is one whole tick of the hot path over one synthetic snapshot (SURVEY.m
 performs of KubeNode.can_fit (kube.py:173) or of a `(x - pod.resources).possible` pool/bin test
 (scaler.py:134,139, capacity.py:30); the count is checked against the oracle's count in the parity tests.
 
-N = 1 (the driver's BENCH line): headline = BASELINE.json configs[1] (c2: 100k pending pods x 10k nodes x 4 dims x
+--dump-outputs DIR (N = 1) writes what the last timed step computed -- the arrays a caller of the tick receives --
+as DIR/<name>.npy in float64; the snapshot is generated from a fixed seed, so two builds compare output for output.
+
+N = 1: headline = BASELINE.json configs[1] (c2: 100k pending pods x 10k nodes x 4 dims x
 1 pool); `configs.c3` and `configs.c5` carry the larger single-GPU configurations (1M x 100k x 8 x 8; the
 idle-node scan over 1M nodes) measured in the same run, each with value / e2e / roofline.
 N > 1 (torchrun, one rank per GPU): ONE cluster -- c3 -- on all ranks in cluster mode (include/acsfit.h): strong
@@ -51,7 +55,7 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 700 W card)"
 
 
 class ClockSampler(object):
@@ -96,9 +100,9 @@ class ClockSampler(object):
         return (int(float(parts[0])), int(float(parts[1])), [p.lower().startswith("active") for p in parts[2:6]])
 
     def _run(self):
-        # Every NVML query takes driver locks that the tick's own launches and copies need: measured on the B200 box, a
-        # 50 ms period put a 10-24 ms outlier into about one c2 step in twenty, a 1 s period none.  So: a first sample
-        # shortly after the timed region starts (the GPU is under load since the warm-up), then four per second.
+        # Every NVML query takes driver locks that the tick's own launches and copies need, so frequent sampling puts
+        # outliers into the timed steps.  So: a first sample shortly after the timed region starts (the GPU is under
+        # load since the warm-up), then four per second.
         if self._stop.wait(0.02):
             return
         while not self._stop.is_set():
@@ -141,17 +145,6 @@ def idle_bytes(R, N, D, S):
 
 def occupancy_bytes(R, N, D):
     return R * 8 * D + 8 * (N + 1) + N * 16 * D
-
-
-def ncu_traffic(name):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture of this round
-    (profiles/r02_traffic.json, written by tools/summarise_profiles.py from the .ncu-rep), or None."""
-    path = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    try:
-        with open(path) as f:
-            return json.load(f).get(name)
-    except Exception:
-        return None
 
 
 # ---------------------------------------------------------------------------------------------
@@ -324,8 +317,17 @@ class Workload(object):
         r = eng.scale_up(d["req"], *self.pool_args(), d["cap_type"], d["node_type"], self.used)  # rows F0, F1, F
         st = eng.node_states(d["row_ptr"], d["run_idx"], d["req_run"], d["flags_run"], d["cap_type"], d["node_type"],
                              d["node_flags"], d["node_age"], r["n_to_schedule"] > 0, self.thr)   # row I (K6)
-        eng.maintain_actions(st[0], d["node_pool"], self.budget, self.scalable, True)            # row J
+        state, action = eng.maintain_actions(st[0], d["node_pool"], self.budget, self.scalable, True)  # row J
+        self.last = (r, state, action)  # references only: read back after the timed steps by --dump-outputs
         return r
+
+    def outputs(self):
+        """what the last step_device returned to its caller, as float64 host arrays (exact for these integers)"""
+        r, state, action = self.last
+        out = {k: r[k] for k in ("feasible", "placed", "acc_pool", "new_size", "units_needed", "bins_opened")}
+        out.update(used=self.used, node_state=state, action=action,
+                   counters=[r[k] for k in ("n_to_schedule", "n_pending", "num_unaccounted", "decisions")])
+        return {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.asarray(v)).astype(np.float64) for k, v in out.items()}
 
     def step_host(self):
         eng, h = self.eng, self.h
@@ -365,9 +367,8 @@ MIN_WARM_SECONDS = 0.25
 
 def timed(step_fn, steps, warmup, flush, barrier, launch_count, min_warm_seconds=0.0):
     import torch
-    # W untimed steps, and (single-process runs: min_warm_seconds > 0) at least that long: the per-step list of the
-    # round-2 runs shows the first one or two timed steps slower than the rest (8.9-9.0 against 8.7 ms, once 16 ms)
-    # when the SM clock is still ramping up from idle after only ~30 ms of load.  (Never time-based under torchrun:
+    # W untimed steps, and (single-process runs: min_warm_seconds > 0) at least that long: the first timed steps run
+    # slower than the rest while the SM clock is still ramping up from idle after a few ms of load.  (Never time-based under torchrun:
     # cluster-mode ticks are collective, every rank must run the same number of them.)
     t_warm = time.perf_counter()
     n_warm = 0
@@ -377,7 +378,7 @@ def timed(step_fn, steps, warmup, flush, barrier, launch_count, min_warm_seconds
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
     # CPython's cyclic GC is paused over the timed steps (as Cluster.loop_logic pauses it over a tick): a generation-2
     # pass over the interpreter's ~10^6 objects (torch is imported) takes 10-30 ms and lands inside some step, between two
-    # launches of the tick - measured as one c3 step in eight at 187 instead of 154 ms.
+    # launches of the tick.
     import gc
     gc.collect()
     gc_was_on = gc.isenabled()
@@ -401,10 +402,10 @@ def timed(step_fn, steps, warmup, flush, barrier, launch_count, min_warm_seconds
     return res, sum(LAST_STEP_MS), launch_count() - l0
 
 
-INT_LANE_OPS_PER_CLK_SM = 77.0  # measured: tools/ubench6.cu, profiles/r02b_ubench6.txt (IADD + LOP3 mix, all SMs busy)
+INT_LANE_OPS_PER_CLK_SM = 76.0  # measured with tools/ubench6.cu on an H100 80GB HBM3 at a 400 W limit (IADD + LOP3 mix, all SMs busy)
 
 
-def physical_roofline(kernel_dec_per_s, nw, sm_mhz, kernel_ms=None, placements=None, sms=148):
+def physical_roofline(kernel_dec_per_s, nw, sm_mhz, sms, kernel_ms=None, placements=None):
     """what actually bounds the pipeline.  (1) The candidate scan is integer-issue work: a pair costs 2 ops per packed
     word + 1 compare (acsfit_kernels.cuh) at the measured int32 issue rate; credited decisions ~ pairs tested.
     (2) Below that ceiling sits the sequential placement chain: first fit is a recurrence, every placement waits for
@@ -414,12 +415,12 @@ def physical_roofline(kernel_dec_per_s, nw, sm_mhz, kernel_ms=None, placements=N
     out = {"achieved": kernel_dec_per_s, "unit": UNIT}
     if nw:
         ops = 2 * nw + 1
-        out["limiter"] = ("the sequential placement chain (see chain_ns_per_placement; a placing step costs ~77 cycles in the "
-                          "frontier warp's loop plus per-batch and per-tile work, and nothing else can proceed past it); the scan's own ceiling is int32 "
+        out["limiter"] = ("the sequential placement chain (see chain_ns_per_placement; every placing step runs in the "
+                          "frontier warp's loop, plus per-batch and per-tile work, and nothing else can proceed past it); the scan's own ceiling is int32 "
                           "issue: %d ops per pair at %d packed word(s) per row" % (ops, nw))
         out["ceiling"] = sms * INT_LANE_OPS_PER_CLK_SM * sm_mhz * 1e6 / ops
         out["frac"] = kernel_dec_per_s / out["ceiling"]
-        out["source"] = "tools/ubench6.cu: %.0f int32 lane-ops/clk/SM (profiles/r02b_ubench6.txt) x SM clock under load" % INT_LANE_OPS_PER_CLK_SM
+        out["source"] = "tools/ubench6.cu: %.0f int32 lane-ops/clk/SM x %d SMs x SM clock under load" % (INT_LANE_OPS_PER_CLK_SM, sms)
     else:
         out["limiter"] = "fp64 compare issue (float64 scan: D DSETP per pair, ~45 lane-ops/clk/SM, tools/ubench5.cu) and the placement chain"
     if kernel_ms and placements:
@@ -447,7 +448,7 @@ def sub_record_c3(eng, syn, flush, steps, peak):
             "e2e": {"value": res["decisions"] * steps / (host_ms * 1e-3), "unit": UNIT, "ms_per_step": host_ms / steps,
                     "h2d_bytes_per_step": int(w.h2d), "d2h_bytes_per_step": int(w.d2h)},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": ncu_traffic("pipeline_c3"), "kernel_ms_per_step": k_ms,
+                         "kernel_ms_per_step": k_ms,
                          "kernel_decisions_per_s": k_dec / (k_ms * 1e-3),
                          "note": "SURVEY 8(d) bytes (64 per decision at D = 8) over the pipeline's kernel time; rows "
                                  "stay on chip, so this exceeds the HBM peak -- see physical"}}, k_dec / (k_ms * 1e-3)
@@ -488,12 +489,12 @@ def sub_record_c5(eng, syn, flush, peak):
             "running_pods": int(R),
             "node_states": {"ms": k6, "nodes_per_s": N / (k6 * 1e-3), "algorithmic_bytes": int(b6),
                             "roofline": {"bound": "hbm", "achieved": b6 / (k6 * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                                         "frac": b6 / (k6 * 1e-3) / 1e9 / peak, "traffic": ncu_traffic("k6_D%d" % D)}},
+                                         "frac": b6 / (k6 * 1e-3) / 1e9 / peak}},
             "occupancy": {"ms": k1, "algorithmic_bytes": int(b1),
                           "roofline": {"bound": "hbm", "achieved": b1 / (k1 * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                                       "frac": b1 / (k1 * 1e-3) / 1e9 / peak, "traffic": ncu_traffic("k1_D%d" % D)}},
+                                       "frac": b1 / (k1 * 1e-3) / 1e9 / peak}},
             "timing": "CUDA events around the Python call (includes the launch and, for node_states, the thresholds' "
-                      "H2D); the ncu kernel durations are in profiles/r02_summary.md"}
+                      "H2D)"}
     out["workload"] = "c5: idle-node scan, %d nodes x ~10 running pods, %d idle thresholds" % (C5_NODES, len(C5_THRESHOLDS))
     return out
 
@@ -548,6 +549,19 @@ def python_surface(eng, syn, c, reps=3):
                     "KubePod / KubeNode construction, flattening, GPU tick, decisions mapped back" % reps}
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, arrays):
+    """DIR/<name>.npy for every array; the largest configuration (c3) writes about 32 MB."""
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit("--dump-outputs: %d bytes exceed the %d byte limit" % (total, DUMP_LIMIT_BYTES))
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a)
+
+
 def run_single(args):
     import torch
     from kubernetes_acs_engine_autoscaler_b200 import build as acs_build
@@ -559,12 +573,15 @@ def run_single(args):
     P, N, D, T = CONFIGS[args.config]
     c = syn.make_cluster(P, N, D, T, seed=SEED)
     w = Workload(eng, c)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=eng.device)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=eng.device)  # > 50 MB L2
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     nb = lambda: torch.cuda.synchronize()  # noqa: E731
     peak, peak_src = load_peaks()
     with ClockSampler(0) as clocks:
         res, dev_ms, launches = timed(w.step_device, args.steps, args.warmup, flush, nb, lambda: eng.launch_count, MIN_WARM_SECONDS)
         step_ms, steps_in_order = sorted(LAST_STEP_MS), [round(x, 3) for x in LAST_STEP_MS]
+        if args.dump_outputs:  # before any later leg reuses the engine's buffers
+            dump_outputs(args.dump_outputs, w.outputs())
         res_h, host_ms, _ = timed(w.step_host, args.steps, max(1, args.warmup // 2), flush, nb, lambda: eng.launch_count, MIN_WARM_SECONDS)
     assert res_h["decisions"] == res["decisions"]
     k_ms, k_dec, k_bytes = w.pipeline_leg(flush, max(1, min(args.steps, 5)))
@@ -589,13 +606,13 @@ def run_single(args):
                    "warm_up": "W untimed steps, continued until %.2f s have passed (SM clock settled)" % MIN_WARM_SECONDS,
                    "parallelism": "1 rank"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic("pipeline_%s" % args.config), "peak_source": peak_src,
+                     "peak_source": peak_src,
                      "kernel": "firstfit_pipeline_kernel (nodes + bins launches)", "kernel_ms_per_step": k_ms,
                      "kernel_decisions_per_s": k_dec / (k_ms * 1e-3),
                      "note": "achieved = SURVEY 8(d) algorithmic bytes (8*D per decision) / kernel time; node and bin "
-                             "rows are held on chip, so real DRAM traffic (`traffic`, ncu) is far below it: the "
-                             "kernel is not HBM-bound, `physical` names what does bound it",
-                     "physical": physical_roofline(k_dec / (k_ms * 1e-3), nw, clk.get("sm_mhz"), k_ms, res["n_to_schedule"])},
+                             "rows are held on chip, so real DRAM traffic is far below it: the kernel is not "
+                             "HBM-bound, `physical` names what does bound it",
+                     "physical": physical_roofline(k_dec / (k_ms * 1e-3), nw, clk.get("sm_mhz"), sms, k_ms, res["n_to_schedule"])},
         "e2e": {"value": res["decisions"] * args.steps / (host_ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": int(w.h2d),
                 "d2h_bytes_per_step": int(w.d2h), "ms_per_step": host_ms / args.steps,
                 "path": "acsfit_occupancy_host + acsfit_scale_up_host + acsfit_maintain_host on pinned host arrays"},
@@ -610,7 +627,8 @@ def run_single(args):
             if args.config != "c3":
                 configs["c3"], c3_rate = sub_record_c3(eng, syn, flush, max(1, min(args.steps, 3)), peak)
                 configs["c3"]["roofline"]["physical"] = physical_roofline(
-                    c3_rate, 0 if nw == 0 else 1, clk.get("sm_mhz"), configs["c3"]["roofline"]["kernel_ms_per_step"], CONFIGS["c3"][0])
+                    c3_rate, 0 if nw == 0 else 1, clk.get("sm_mhz"), sms, configs["c3"]["roofline"]["kernel_ms_per_step"],
+                    CONFIGS["c3"][0])
             configs["c5"] = sub_record_c5(eng, syn, flush, peak)
             if args.config == "c2":
                 line["e2e"]["python_surface"] = python_surface(eng, syn, c)
@@ -804,8 +822,11 @@ def main():
     ap.add_argument("--no-c4", action="store_true", help="N > 1: skip the configs.c4 sub-record (10M x 1M, ~1 minute)")
     ap.add_argument("--no-c4-verify", action="store_true", help="skip the single-GPU check of c4 (tens of seconds)")
     ap.add_argument("--no-fleet", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="N = 1: write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.dump_outputs and (world > 1 or args.impl != "ours"):
+        ap.error("--dump-outputs needs --impl ours on one GPU")
     if args.impl == "reference":
         run_reference(args)
         return

@@ -1,5 +1,5 @@
 /*
- * acsfit.h -- C ABI of libacsfit.so, the B200 (sm_100a) decision engine behind the
+ * acsfit.h -- C ABI of libacsfit.so, the H100 (sm_90a) decision engine behind the
  * acs-engine autoscaler's per-tick hot path.
  *
  * The reference (wbuchwalter/Kubernetes-acs-engine-autoscaler) is pure Python and has no
@@ -89,7 +89,7 @@ typedef void *acsfit_stream_t;
 ACSFIT_API int acsfit_abi_version(void);
 ACSFIT_API const char *acsfit_last_error(const acsfit_ctx *ctx);
 
-/* `device` is the CUDA device ordinal.  Fails (ACSFIT_E_CUDA) when no sm_100 device is there:
+/* `device` is the CUDA device ordinal.  Fails (ACSFIT_E_CUDA) when no sm_90 device is there:
  * there is no CPU fallback. */
 ACSFIT_API acsfit_status acsfit_ctx_create(int device, acsfit_ctx **out_ctx);
 ACSFIT_API acsfit_status acsfit_ctx_destroy(acsfit_ctx *ctx);
@@ -99,8 +99,7 @@ ACSFIT_API acsfit_status acsfit_ctx_destroy(acsfit_ctx *ctx);
  *   ACSFIT_OVERLAP=0        do not chain the first bin pass behind the node pass on a second stream
  *   ACSFIT_PRUNE=0|1        never / always use the scan-list-pruning instantiation of the node pass
  *                           (default: only when the pass has more stages than the GPU holds at once)
- *   ACSFIT_MIN_STAGES=n     same as acsfit_ctx_configure(min_stages) (default: one stage per SM; measured best
- *                           for the chained c2 tick as well: 148 -> 10.86 ms, 79 -> 11.13, 40 -> 11.4)
+ *   ACSFIT_MIN_STAGES=n     same as acsfit_ctx_configure(min_stages) (default: one stage per SM)
  *   ACSFIT_SMEM_FLOOR_KB=n  request at least n KB of shared memory per stage CTA (limits CTAs per SM)
  *   ACSFIT_STREAM_BYTES=n   staging bytes per warp of the K1/K6 streaming kernels (2048 / 4096 / 8192)
  *   ACSFIT_RANKS=0          never use the packed-rank scan (float64 compares instead; same results) */

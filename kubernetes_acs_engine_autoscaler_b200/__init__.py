@@ -1,7 +1,7 @@
-"""acsfit: B200-native decision engine behind the acs-engine autoscaler's per-tick hot path.
+"""acsfit: H100-native decision engine behind the acs-engine autoscaler's per-tick hot path.
 
 Host-side mirror of the reference's `autoscaler` package for that path (same class and
-function names), with the arithmetic done by hand-written sm_100a kernels in libacsfit.so.
+function names), with the arithmetic done by hand-written sm_90a kernels in libacsfit.so.
 Importing the package does not load CUDA; constructing an engine does, and fails loudly
 when the extension or a GPU is missing (there is no CPU fallback).
 """

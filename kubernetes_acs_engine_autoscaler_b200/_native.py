@@ -63,7 +63,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 "%s is missing: build it with `python -m kubernetes_acs_engine_autoscaler_b200.build` "
-                "(nvcc, sm_100a). The pod-fit path has no CPU fallback." % LIB_PATH)
+                "(nvcc, sm_90a). The pod-fit path has no CPU fallback." % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         for name, (restype, argtypes) in SIGNATURES.items():
             fn = getattr(lib, name)  # AttributeError if the ABI is incomplete

@@ -1,4 +1,4 @@
-"""Build libacsfit.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libacsfit.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m kubernetes_acs_engine_autoscaler_b200.build
 
@@ -16,7 +16,7 @@ SOURCES = ["acsfit.cu"]
 HEADERS = ["acsfit_kernels.cuh", "acsfit_math.cuh", "acsfit_rank.cuh", "acsfit_stream.cuh", "acsfit_stream_ff.cuh", os.path.join("..", "..", "include", "acsfit.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false",  # 0.3*cap - util must stay a multiply followed by a subtract (scaler.py:86-87)
     "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden",

@@ -1,4 +1,4 @@
-// acsfit.cu -- C ABI (include/acsfit.h) over the sm_100a kernels in acsfit_kernels.cuh.
+// acsfit.cu -- C ABI (include/acsfit.h) over the sm_90a kernels in acsfit_kernels.cuh.
 // Host orchestration only: argument checks, scratch arena, launches, the per-pool loop of
 // fulfill_pending.  There is no CPU implementation of any computation in this file: without a
 // CUDA device acsfit_ctx_create fails and nothing else can be called.
@@ -394,7 +394,7 @@ __global__ void node_states_kernel(const int64_t *__restrict__ row_ptr, const in
 // access pattern changes (coalesced streaming instead of one scattered row per thread).
 constexpr int kStreamWarps = 8;
 static int g_trace = 0;           // ACSFIT_TRACE=1: per-pass timings on stderr (with acsfit_ctx_set_timing)
-static int g_bulk_cfg = 1;        // geometry of the bulk-copy form (developer knob ACSFIT_BULK_CFG)
+static int g_bulk_cfg = 4;        // geometry of the bulk-copy form (developer knob ACSFIT_BULK_CFG)
 static int g_stream_bytes = 8192;  // staging bytes per warp (developer knob ACSFIT_STREAM_BYTES: 2048 / 4096 / 8192)
 
 template <int D, bool STATES, int kStreamBytesPerWarp>
@@ -606,7 +606,7 @@ static cudaError_t launch_node_stream(int grid, cudaStream_t st, const int64_t *
                                       int64_t N, int any_pending, const int64_t *thr, int S, uint8_t *out_state,
                                       double *used)
 {
-    if (!run_idx) {  // contiguous table: Blackwell bulk copies (acsfit_stream.cuh); geometry = <bytes per warp, warps>
+    if (!run_idx) {  // contiguous table: TMA bulk copies (acsfit_stream.cuh); geometry = <bytes per warp, warps>
 #define ACSFIT_BULK_ARGS grid, st, row_ptr, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr, S, out_state, used
         if constexpr (D <= 8) {
             switch (g_bulk_cfg) {
@@ -615,7 +615,7 @@ static cudaError_t launch_node_stream(int grid, cudaStream_t st, const int64_t *
             case 3: return launch_node_stream_bulk<D, STATES, 32768, 6>(ACSFIT_BULK_ARGS);
             case 4: return launch_node_stream_bulk<D, STATES, 8192, 16>(ACSFIT_BULK_ARGS);
             case 0: return launch_node_stream_bulk<D, STATES, 8192, 8>(ACSFIT_BULK_ARGS);
-            default: return launch_node_stream_bulk<D, STATES, 16384, 12>(ACSFIT_BULK_ARGS);  // measured best (profiles/r02_summary.md)
+            default: return launch_node_stream_bulk<D, STATES, 8192, 16>(ACSFIT_BULK_ARGS);  // measured best on H100 (DESIGN.md section 6)
             }
         } else {
             return launch_node_stream_bulk<D, STATES, 16384, 8>(ACSFIT_BULK_ARGS);
@@ -751,9 +751,9 @@ extern "C" acsfit_status acsfit_ctx_create(int device, acsfit_ctx **out_ctx)
     ctx->device = device;
     cudaDeviceProp prop;
     if (cudaSetDevice(device) != cudaSuccess || cudaGetDeviceProperties(&prop, device) != cudaSuccess ||
-        prop.major < 10) {
+        prop.major != 9 || prop.minor != 0) {
         delete ctx;
-        return ACSFIT_E_CUDA;  // built for sm_100a only
+        return ACSFIT_E_CUDA;  // built for sm_90a only
     }
     ctx->num_sms = prop.multiProcessorCount;
     if (cudaEventCreate(&ctx->ev0) != cudaSuccess || cudaEventCreate(&ctx->ev1) != cudaSuccess) {
@@ -1057,8 +1057,8 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     constexpr int NT = stage_threads(D, BINS);
     size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW>::bytes(pp.Tn);
     // D >= 8: ONE stage CTA per SM.  Whether two fit is an accident of the register allocation (the bins kernel has
-    // been compiled to 128 and to 237 registers by neighbouring source revisions); measured at c3, a second CTA on the
-    // frontier's SM costs the placement chain more than the extra resident stages give back (bins 89 -> 76 ms).
+    // been compiled to 128 and to 237 registers by neighbouring source revisions); at c3 a second CTA on the
+    // frontier's SM costs the placement chain more than the extra resident stages give back.
     if (D >= 8) smem = std::max(smem, (size_t)kOneCtaSmemKb * 1024);
     if (ctx->smem_floor_kb > 0) smem = std::max(smem, (size_t)ctx->smem_floor_kb * 1024);  // occupancy knob
     auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW>;
@@ -1113,8 +1113,7 @@ static acsfit_status launch_pipeline_t(acsfit_ctx *ctx, const PipelineParams &pp
     if (!BINS) {
         // Stage bounds + scan-list pruning (the PRUNE instantiation) pay when the pass is throughput-bound, i.e.
         // when there are more stages than the GPU holds at once (waves); a pass that fits is bound by its
-        // placement chain and runs the plain instantiation (measured: c3 nodes pass 143 -> 128 ms with pruning,
-        // c2 tick 10.75 -> 10.93 ms).  ACSFIT_PRUNE=0/1 forces either.
+        // placement chain and runs the plain instantiation.  ACSFIT_PRUNE=0/1 forces either.
         int prune = ctx->prune;
         if (prune != 1 && stream_form_ok(ctx, D, pp.rk.nw, pp.Tn)) prune = 0;  // the streaming form has no pruning variant
         if (prune < 0) {

@@ -1,4 +1,4 @@
-// acsfit_kernels.cuh -- sm_100a kernels of the pod-fit path (no tensor cores: this is
+// acsfit_kernels.cuh -- sm_90a kernels of the pod-fit path (no tensor cores: this is
 // compare / reduce work on float64, see DESIGN.md).
 //
 // The centrepiece is firstfit_pipeline_kernel: an EXACT, order-preserving parallelisation of

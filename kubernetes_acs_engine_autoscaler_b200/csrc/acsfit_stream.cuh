@@ -3,9 +3,9 @@
 // same ordered float64 sums as node_stream_kernel (acsfit.cu); what changes is how bytes reach the SM:
 //
 //   * a warp owns a contiguous range of 32-node groups, hence ONE contiguous byte range of req_run / flags_run.
-//     It streams that range through two shared-memory buffers with Blackwell bulk copies: one
+//     It streams that range through two shared-memory buffers with Hopper TMA bulk copies: one
 //     `cp.async.bulk.shared.global` per chunk for the rows and one for the flag bytes, issued by a single lane and
-//     completed on an mbarrier (SASS: UBLKCP + SYNCS) -- no per-lane address arithmetic, no index gather, no
+//     completed on an mbarrier -- no per-lane address arithmetic, no index gather, no
 //     16-byte cp.async fan-out;
 //   * chunk boundaries are multiples of 16 entries from the start of the table, so every copy is 16-byte aligned
 //     in global and shared memory (the first chunk may start a few entries before the warp's range: ignored);
@@ -20,11 +20,10 @@ namespace acsfit {
 
 // Lane = node: a warp is only fully busy while the chunk in shared memory holds entries of all 32 nodes of the
 // group it is summing.  With ~10 running pods per node that takes >= 320 entries per chunk, so the chunks are
-// large (16 KB per buffer, two buffers per warp) and the CTA has few warps: 6 x 32 KB = 192 KB of staging per SM,
-// all of it in flight.  (ncu of the first version, 4 KB chunks and 8 warps: 6 of 32 lanes active on average in
-// the consume loop, 60 % of the issue slots busy at 0.55 of the HBM peak -- issue-bound on idle lanes.)
+// large and the CTA has few warps; with small chunks the consume loop is issue-bound on idle lanes.
 // The two pull against each other (fewer warps hide less latency), so the geometry is a template pair
-// <warps per CTA, staging bytes per warp> chosen per kernel from measurements (profiles/r02_summary.md).
+// <warps per CTA, staging bytes per warp> chosen from measurements on H100 (DESIGN.md section 6): 16 warps x 8 KB
+// = 128 KB of staging per SM, all of it in flight.
 
 __device__ __forceinline__ void mbar_init(uint64_t *bar, unsigned count)
 {

@@ -5,8 +5,8 @@
 // parallel candidate scan in rank space is followed by an in-order resolve through a chain of warps (warp w owns
 // nodes 32w..32w+31 of the stage, lane = node, literal float64 reference expression).  What changes is the
 // schedule inside the CTA.  In the barrier form every tile is load -> scan -> resolve -> refresh -> publish with
-// __syncthreads between the phases, so the warp chain DRAINS before the next tile may enter it: a frontier tile of
-// config 2 costs 27-45 k cycles although its busiest warp works 10-14 k (profiles/r02_summary.md).  Here every warp
+// __syncthreads between the phases, so the warp chain DRAINS before the next tile may enter it: a frontier tile
+// costs several times the work of its busiest warp.  Here every warp
 // runs its own loop and tiles stream through the chain:
 //
 //   warp w, iteration i:   scan share of tile i      (its 32 pods against ALL nodes of the stage, packed ranks)
@@ -418,10 +418,9 @@ firstfit_stream_kernel(const PipelineParams p)
                         }
                         return ok & ok2;
                     };
-                    // Measured (profiles/r02_summary.md): bins at D = 8 102 -> 84 ms (c3).  Not used where it loses: the D = 8
-                    // node test is 24 float64 instructions per entry and issue-bound (c3 nodes 98 -> 106 ms with it); at
-                    // D <= 4 the extra registers (122 -> 148) cost the second stage CTA per SM, and with it the
-                    // nodes -> bins chaining of the c2 tick (10.7 -> 10.9 ms; capped at 128 registers: 11.6 ms).
+                    // It pays for the bins at D = 8.  Not used where it loses: the D = 8 node test is 24 float64
+                    // instructions per entry and issue-bound; at D <= 4 the extra registers cost the second stage CTA
+                    // per SM, and with it the nodes -> bins chaining of the c2 tick.
                     constexpr bool kSpeculate = BINS && D >= 8;
                     if constexpr (!kSpeculate) {
                         for (int k0 = 0; k0 < n_poss; k0 += 4)

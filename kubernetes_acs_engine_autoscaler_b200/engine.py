@@ -1,7 +1,7 @@
 """Device engine: thin Python face of libacsfit.so on dense float64 snapshots.
 
 PyTorch is only the buffer container here (device memory, streams); every computation is a
-hand-written sm_100a kernel behind the C ABI of include/acsfit.h.  There is no CPU
+hand-written sm_90a kernel behind the C ABI of include/acsfit.h.  There is no CPU
 implementation: constructing an Engine without a CUDA device raises.
 """
 import ctypes
@@ -44,7 +44,7 @@ class Engine(object):
     def __init__(self, device=None, min_stages=0, watchdog_ms=0):
         self._lib = _native.load()
         if not torch.cuda.is_available():
-            raise RuntimeError("acsfit needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("acsfit needs a CUDA device (sm_90a); there is no CPU fallback")
         if device is None:
             device = torch.cuda.current_device()
         self.device = torch.device("cuda", int(device))

@@ -7,10 +7,11 @@ hot path (SURVEY.md section 8c), so empty stand-ins are enough to import
 `autoscaler.cluster`, `autoscaler.scaler`, `autoscaler.engine_scaler`,
 `autoscaler.kube`, `autoscaler.capacity` exactly as they lie on disk.
 
-This module only works where `/root/reference` exists (the build container).
-It is used by `oracle/make_golden.py` to generate the committed fixtures under
-`tests/golden/`, and by the optional differential tests that are skipped when
-the reference tree is missing (the GPU box).  Nothing in the product imports it.
+This module only works where the reference tree is present ($ACSFIT_REFERENCE_ROOT, or
+the copy oracle/build_ref.py staged in oracle/_ref).  It is used by
+`oracle/make_golden*.py` to record the committed fixtures under `tests/golden/`
+that the differential tests compare against, and by bench.py's CPU baseline.
+Nothing in the product imports it.
 """
 import importlib
 import json

@@ -6,6 +6,7 @@ import datetime
 import gzip
 import json
 import logging
+import lzma
 import os
 from collections import OrderedDict
 
@@ -16,6 +17,9 @@ def load_json(name):
     path = os.path.join(GOLDEN, name)
     if name.endswith(".gz"):
         with gzip.open(path, "rt") as f:
+            return json.load(f)
+    if name.endswith(".xz"):
+        with lzma.open(path, "rt") as f:
             return json.load(f)
     with open(path) as f:
         return json.load(f)

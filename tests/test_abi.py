@@ -1,4 +1,4 @@
-"""`-m "not gpu"`: libacsfit.so builds (nvcc cross-compiles sm_100a without a GPU), loads, and exports
+"""`-m "not gpu"`: libacsfit.so builds (nvcc cross-compiles sm_90a without a GPU), loads, and exports
 every symbol include/acsfit.h declares; the product refuses to run without CUDA."""
 import ctypes
 import os
@@ -30,11 +30,12 @@ def test_library_exports_every_declared_symbol():
     assert set(names) <= set(_native.SIGNATURES)
 
 
-def test_built_for_sm_100a_only():
+def test_built_for_sm_90a_only():
     from kubernetes_acs_engine_autoscaler_b200 import build as acs_build
-    out = subprocess.run(["cuobjdump", "--list-elf", acs_build.build()], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert not re.search(r"sm_(?!100a)\d+", out)
+    cuobjdump = os.path.join(os.path.dirname(acs_build._nvcc()), "cuobjdump")
+    out = subprocess.run([cuobjdump, "--list-elf", acs_build.build()], capture_output=True, text=True).stdout
+    assert "sm_90a" in out
+    assert not re.search(r"sm_(?!90a)\d+", out)
 
 
 def test_no_cpu_fallback():

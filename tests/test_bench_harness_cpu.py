@@ -79,6 +79,17 @@ def test_gc_is_restored_when_a_step_raises(bench, fake_cuda):
     assert gc.isenabled()
 
 
+def test_dump_outputs_writes_npy_and_caps_the_total(bench, tmp_path):
+    import numpy as np
+    a = {"placed": np.arange(5, dtype=np.float64) - 2, "used": np.ones((3, 4))}
+    bench.dump_outputs(str(tmp_path / "out"), a)
+    for k, v in a.items():
+        np.testing.assert_array_equal(np.load(str(tmp_path / "out" / (k + ".npy"))), v)
+    with pytest.raises(SystemExit):
+        bench.dump_outputs(str(tmp_path / "big"), {"x": np.zeros(bench.DUMP_LIMIT_BYTES // 8 + 1)})
+    assert not (tmp_path / "big").exists()
+
+
 def test_clock_sampler_without_nvml_or_nvidia_smi_reports_nothing(bench):
     if torch.cuda.is_available():
         pytest.skip("a GPU is present: the sampler has something to report")

@@ -29,16 +29,25 @@ def test_c2_full_tick_matches_oracle(engine, oracle_mod):
     assert o["decisions"] > 1.5e9  # the configuration the metric is quoted on
 
 
-def test_c3_shaped_tick_matches_oracle_exactly(engine, oracle_mod, request):
+_C3_SHAPED = {}
+
+
+def c3_shaped_oracle(oracle_mod):
+    """the snapshot and the oracle's answer, computed once per process (the oracle needs about a minute) and shared by
+    every engine mode"""
+    if not _C3_SHAPED:
+        c = syn.make_cluster(500000, 50000, 8, 8, seed=20260925)
+        used0 = syn.initial_used(c)
+        used_o = used0.copy()
+        _C3_SHAPED.update(c=c, used0=used0, o=oracle_scale_up(oracle_mod, c, used_o), used_o=used_o)
+    return _C3_SHAPED["c"], _C3_SHAPED["used0"], _C3_SHAPED["o"], _C3_SHAPED["used_o"]
+
+
+def test_c3_shaped_tick_matches_oracle_exactly(engine, oracle_mod):
     """BASELINE config 3's SHAPE (8 dims, 8 pools, multi-wave node pass, several bin passes and pools) at half its
-    size -- 500 k pods x 50 k nodes, about 30 G reference decisions -- compared EXACTLY with the plain-C oracle (which
-    needs about a minute for it; run once, for the default engine mode only)."""
-    if "ranks" not in request.node.callspec.id:
-        pytest.skip("one engine mode is enough for the one-minute oracle run (the other modes run every smaller case)")
-    c = syn.make_cluster(500000, 50000, 8, 8, seed=20260925)
-    used0 = syn.initial_used(c)
-    used_o = used0.copy()
-    o = oracle_scale_up(oracle_mod, c, used_o)
+    size -- 500 k pods x 50 k nodes, about 30 G reference decisions -- compared EXACTLY with the plain-C oracle, in
+    every engine mode."""
+    c, used0, o, used_o = c3_shaped_oracle(oracle_mod)
     f64, i32 = torch.float64, torch.int32
     d_used = engine.dev(used0, f64)
     g = engine.scale_up(engine.dev(c["req"], f64), c["unit_all"], c["unit_ordered"], c["pool_actual"], c["pool_max"],

@@ -1,5 +1,5 @@
 """`-m gpu`: the reference's recorded ticks and known-answer tests through the product's public
-classes with the REAL CUDA engine (C ABI -> sm_100a kernels): exceptions, scale_pools arguments,
+classes with the REAL CUDA engine (C ABI -> sm_90a kernels): exceptions, scale_pools arguments,
 used_capacity bit patterns, node states, adapter calls and the complete log text must match."""
 import pytest
 

@@ -1,20 +1,16 @@
-"""`-m "not gpu"`, only where the reference is present: the HOST LAYER of this package (Cluster.loop_logic: object
-construction incl. the C helper, flattening, hand-off, write-back of `used_capacity`, maintain) on mid-size synthetic
-clusters against the unmodified reference run live on the same kube-style objects.  The device work is done by the
-plain-C oracle here (tests/oracle_engine.py); the CUDA engine behind the same layer is checked by the GPU suite."""
+"""`-m "not gpu"`: the HOST LAYER of this package (Cluster.loop_logic: object construction incl. the C helper,
+flattening, hand-off, write-back of `used_capacity`, maintain) on mid-size synthetic clusters against what the
+unmodified reference computed on the same kube-style objects (recorded in tests/golden/live_reference.json.xz by
+oracle/make_golden_live.py).  The device work is done by the plain-C oracle here (tests/oracle_engine.py); the CUDA
+engine behind the same layer is checked by the GPU suite."""
 import logging
-import os
 import re
-import sys
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "oracle"))
-import ref_shim  # noqa: E402
-
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present")
+import golden_util as gu
+import mid_golden
 
 
 class Raw(object):
@@ -46,14 +42,13 @@ def test_loop_logic_equals_the_live_reference(oracle_mod, tmp_path, monkeypatch,
     from kubernetes_acs_engine_autoscaler_b200 import synthetic as syn
     from kubernetes_acs_engine_autoscaler_b200.cluster import Cluster
 
-    c = syn.make_cluster(P, N, D, T, seed=seed, over_provision=1)
+    # ---- the reference, recorded ----------------------------------------------------------------
+    ref = [r for r in gu.load_json("live_reference.json.xz")["host_layer"]
+           if (r["P"], r["N"], r["D"], r["T"], r["seed"], r["max_size"]) == (P, N, D, T, seed, max_size)][0]
+    c = mid_golden.cluster_of({"P": P, "N": N, "D": D, "T": T, "seed": seed, "over_provision": 1, "digest": ref["digest"]})
     cap = int(max_size if max_size is not None else c["pool_max"][0])
-
-    # ---- the reference, live -------------------------------------------------------------------
-    tick = ref_bench.ReferenceTick(c, tmpdir=str(tmp_path), max_size=cap)
-    ref = tick.run(record=True)
-    ref_keys = [set(n.used_capacity.raw) for n in tick.nodes]
-    ref_state = {n.name: s for n, s in zip(tick.nodes, ref["states"])}
+    ref_keys = [set(k) for k in ref["used_keys"]]
+    ref_state = dict(zip(ref["node_names"], ref["states"]))
 
     # ---- this package's host layer on the same objects -----------------------------------------
     st = syn.kube_objects(c)
@@ -104,13 +99,13 @@ def test_loop_logic_equals_the_live_reference(oracle_mod, tmp_path, monkeypatch,
         assert exc[0] == ref["exception"][0]
     assert scale_calls == ref["scale_calls"]
     names = c["dim_names"]
-    assert [n.name for n in kube_nodes] == [n.name for n in tick.nodes]
+    assert [n.name for n in kube_nodes] == ref["node_names"]
     used = np.array([[float(n.used_capacity.raw.get(k, 0.0)) for k in names] for n in kube_nodes], dtype=np.float64)
-    assert np.array_equal(used.view(np.uint64), ref["used"].view(np.uint64))
+    assert np.array_equal(used.view(np.uint64), mid_golden._unpack(ref["used_bits"], np.uint64).reshape(N, D))
     assert [set(n.used_capacity.raw) for n in kube_nodes] == ref_keys      # KubeResource.__add__ unions the key sets
     text = "\n".join(handler.lines)
-    assert "Pods to schedule: %d" % len(ref["to_schedule"]) in text
-    assert "Pending pods: %d" % len(ref["pending"]) in text
+    assert "Pods to schedule: %d" % ref["n_to_schedule"] in text
+    assert "Pending pods: %d" % ref["n_pending"] in text
     if exc is None:  # maintain ran: one state line per node of a scalable pool, the reference's state strings
         got_state = {}
         for line in handler.lines:
@@ -118,4 +113,4 @@ def test_loop_logic_equals_the_live_reference(oracle_mod, tmp_path, monkeypatch,
             if m:
                 got_state[re.search(r"(k8s-[a-z0-9]+-\d+-\d+)", m.group(1)).group(1)] = m.group(2)
         assert len(got_state) == len(kube_nodes)
-        assert got_state == {k: str(v) for k, v in ref_state.items()}
+        assert got_state == ref_state

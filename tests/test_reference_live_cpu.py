@@ -1,45 +1,42 @@
-"""`-m "not gpu"`, only where the reference is present (/root/reference in the build container, or the staged
-oracle/_ref that travels with the snapshot): the reference's own constructors give the synthetic dense rows back
-bit for bit (SURVEY.md section 7), and the C oracle equals the live reference on a mid-size tick."""
-import os
-import sys
-
+"""`-m "not gpu"`: the reference's own constructors give the synthetic dense rows back bit for bit (SURVEY.md
+section 7), and the C oracle equals the reference on a mid-size tick.  What the unmodified reference computed is
+recorded in tests/golden/live_reference.json.xz (oracle/make_golden_live.py)."""
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "oracle"))
-import ref_shim  # noqa: E402
+import golden_util as gu
+import mid_golden
+from kubernetes_acs_engine_autoscaler_b200 import synthetic as syn
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present")
+
+def golden():
+    return gu.load_json("live_reference.json.xz")
 
 
 @pytest.mark.parametrize("D,T", [(4, 1), (8, 8)])
-def test_synthetic_rows_equal_reference_constructors(tmp_path, D, T):
-    import ref_bench
-    from kubernetes_acs_engine_autoscaler_b200 import synthetic as syn
-    c = syn.make_cluster(400, 40, D, T, seed=77)
-    tick = ref_bench.ReferenceTick(c, tmpdir=str(tmp_path))
+def test_synthetic_rows_equal_reference_constructors(D, T):
+    rec = [r for r in golden()["rows"] if (r["D"], r["T"]) == (D, T)][0]
+    c = mid_golden.cluster_of({"P": 400, "N": 40, "D": D, "T": T, "seed": 77, "digest": rec["digest"]})
     names = c["dim_names"]
-    pending = [p for p in tick.pods if p.status == "Pending"]
-    assert len(pending) == c["P"] and len(tick.running) == c["req_run"].shape[0]
-    for p, row in zip(pending, c["req"]):        # KubePod.resources (kube.py:41-49) == the dense request row
-        got = np.array([float(p.resources.raw.get(k, 0.0)) for k in names])
-        assert np.array_equal(got.view(np.uint64), row.view(np.uint64)) and set(p.resources.raw) <= set(names)
-    for p, row in zip(tick.running, c["req_run"][c["run_idx"]]):
-        got = np.array([float(p.resources.raw.get(k, 0.0)) for k in names])
-        assert np.array_equal(got.view(np.uint64), row.view(np.uint64))
-    for n, t in zip(tick.nodes, c["node_type"]):  # create_kube_node capacity (cluster.py:130-133) == cap_type row
-        got = np.array([float(n.capacity.raw.get(k, 0.0)) for k in names])
-        assert np.array_equal(got.view(np.uint64), c["cap_type"][t].view(np.uint64))
-    tick.occupancy()                               # count_pod sums (cluster.py:165-168) == initial_used
-    used = np.array([[float(n.used_capacity.raw.get(k, 0.0)) for k in names] for n in tick.nodes])
-    assert np.array_equal(used.view(np.uint64), syn.initial_used(c).view(np.uint64))
+    assert rec["n_pending"] == c["P"] and rec["n_running"] == c["req_run"].shape[0]
+    assert set(rec["pending_keys"]) <= set(names)
+
+    def bits(key, rows):
+        return mid_golden._unpack(rec[key], np.uint64).reshape(rows, len(names))
+    # KubePod.resources (kube.py:41-49) == the dense request rows, running and pending
+    np.testing.assert_array_equal(bits("pending_bits", c["P"]), c["req"].view(np.uint64))
+    np.testing.assert_array_equal(bits("running_bits", rec["n_running"]), c["req_run"][c["run_idx"]].view(np.uint64))
+    # create_kube_node capacity (cluster.py:130-133) == cap_type row
+    np.testing.assert_array_equal(bits("capacity_bits", c["N"]), c["cap_type"][c["node_type"]].view(np.uint64))
+    # count_pod sums (cluster.py:165-168) == initial_used
+    np.testing.assert_array_equal(bits("used_bits", c["N"]), syn.initial_used(c).view(np.uint64))
 
 
-def test_oracle_equals_live_reference(oracle_mod, tmp_path):
+def test_oracle_equals_live_reference(oracle_mod):
     import ref_bench
-    from kubernetes_acs_engine_autoscaler_b200 import synthetic as syn
-    c = syn.make_cluster(700, 90, 8, 8, seed=78, over_provision=1)
-    res = ref_bench.ReferenceTick(c, tmpdir=str(tmp_path)).run()
+    rec = golden()["oracle_tick"]
+    c = mid_golden.cluster_of({k: rec[k] for k in ("P", "N", "D", "T", "seed", "digest")} | {"over_provision": 1})
+    res = {"to_schedule": rec["to_schedule"], "pending": rec["pending"], "scale_calls": rec["scale_calls"],
+           "exception": rec["exception"],
+           "used": mid_golden._unpack(rec["used_bits"], np.uint64).reshape(c["N"], c["D"]).view(np.float64)}
     assert ref_bench.compare(c, res, ref_bench.dense_answer(oracle_mod, c)) == []

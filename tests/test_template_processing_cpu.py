@@ -1,20 +1,12 @@
 """ARM template unrolling (SURVEY.md section 8(f)3): the reference's own known-answer tests
-(test/test_template_processing.py:34-89) and, where the reference is present, a differential run of every
-function on the reference's fixture templates."""
+(test/test_template_processing.py:34-89) and a differential run of every function against the reference's
+recorded results on its fixture templates."""
 import copy
-import json
-import os
-import sys
 
 import pytest
 
+import golden_util as gu
 from kubernetes_acs_engine_autoscaler_b200 import template_processing as tp
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "oracle"))
-import ref_shim  # noqa: E402
-
-REF_DATA = os.path.join(ref_shim.REFERENCE_ROOT, "test", "data")
 
 
 class Node(object):
@@ -94,38 +86,40 @@ def test_scale_out_template_shape():
     assert len(tp.delete_master_vm_extension(mini_template())["resources"]) == len(mini_template()["resources"]) - 1
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_DATA) or not ref_shim.available(), reason="reference fixtures not present")
-def test_every_function_equals_the_reference_on_its_fixtures():
-    ns = ref_shim.load_reference()
-    import importlib
-    sys.path.insert(0, ref_shim.REFERENCE_ROOT)
-    try:
-        ref_tp = importlib.import_module("autoscaler.template_processing")
-    finally:
-        sys.path.remove(ref_shim.REFERENCE_ROOT)
-    del ns
+def fixture_pool_names(cluster):
+    return sorted({r["name"].split("variables('")[1].split("VMNamePrefix")[0] for r in cluster["resources"]
+                   if "VMNamePrefix'), copyIndex" in r["name"] and "master" not in r["name"]})
 
-    def load(name):
-        with open(os.path.join(REF_DATA, name)) as f:
-            return json.load(f)
-    original = load("azuredeploy.original.json")
-    pool = Pool("agentpool1", [0])
-    # the reference's two fixture KATs (test/test_template_processing.py:34-56)
-    assert tp.unroll_nic(copy.deepcopy(original), pool, 3) == load("azuredeploy.expected_nic.json")
-    assert tp.unroll_vm(copy.deepcopy(original), pool, 3) == load("azuredeploy.expected_vm.json")
-    cluster = load("azuredeploy.cluster.json")
-    pool_names = sorted({r["name"].split("variables('")[1].split("VMNamePrefix")[0] for r in cluster["resources"]
-                         if "VMNamePrefix'), copyIndex" in r["name"] and "master" not in r["name"]})
-    assert pool_names
+
+def template_calls(pool_names):
+    """every function on the reference's cluster fixture: call(module, template copy, Pool class) -> result.
+    oracle/make_golden_live.py records the reference's results of exactly these calls."""
+    calls = []
     for sizes, held in [({n: 3 for n in pool_names}, [0]), ({n: 1 for n in pool_names}, [0]),
                         ({n: (5 if i == 0 else 2) for i, n in enumerate(pool_names)}, [1, 3])]:
-        pools = [Pool(n, held) for n in pool_names]
-        assert tp.prepare_template_for_scale_out(copy.deepcopy(cluster), pools, dict(sizes)) == \
-            ref_tp.prepare_template_for_scale_out(copy.deepcopy(cluster), pools, dict(sizes))
+        calls.append(lambda m, t, P, sizes=sizes, held=held:
+                     m.prepare_template_for_scale_out(t, [P(n, held) for n in pool_names], dict(sizes)))
     for fn in ("unroll_vm_extension", "unroll_nic", "unroll_vm"):
-        assert getattr(tp, fn)(copy.deepcopy(cluster), Pool(pool_names[0], [0, 2]), 5) == \
-            getattr(ref_tp, fn)(copy.deepcopy(cluster), Pool(pool_names[0], [0, 2]), 5)
-    assert tp.delete_master_vm_extension(copy.deepcopy(cluster)) == ref_tp.delete_master_vm_extension(copy.deepcopy(cluster))
-    assert tp.delete_nsg(cluster) == ref_tp.delete_nsg(cluster)
-    assert tp.delete_unchanged_pools(copy.deepcopy(cluster), [Pool(pool_names[0], [0])]) == \
-        ref_tp.delete_unchanged_pools(copy.deepcopy(cluster), [Pool(pool_names[0], [0])])
+        calls.append(lambda m, t, P, fn=fn: getattr(m, fn)(t, P(pool_names[0], [0, 2]), 5))
+    calls.append(lambda m, t, P: m.delete_master_vm_extension(t))
+    calls.append(lambda m, t, P: m.delete_nsg(t))
+    calls.append(lambda m, t, P: m.delete_unchanged_pools(t, [P(pool_names[0], [0])]))
+    return calls
+
+
+def test_every_function_equals_the_reference_on_its_fixtures():
+    """the reference's fixture templates and its results on them, recorded in tests/golden/live_reference.json.xz"""
+    rec = gu.load_json("live_reference.json.xz")["templates"]
+    files = rec["files"]
+    original = files["azuredeploy.original.json"]
+    pool = Pool("agentpool1", [0])
+    # the reference's two fixture KATs (test/test_template_processing.py:34-56)
+    assert tp.unroll_nic(copy.deepcopy(original), pool, 3) == files["azuredeploy.expected_nic.json"]
+    assert tp.unroll_vm(copy.deepcopy(original), pool, 3) == files["azuredeploy.expected_vm.json"]
+    cluster = files["azuredeploy.cluster.json"]
+    pool_names = fixture_pool_names(cluster)
+    assert pool_names
+    calls = template_calls(pool_names)
+    assert len(calls) == len(rec["results"])
+    for call, want in zip(calls, rec["results"]):
+        assert call(tp, copy.deepcopy(cluster), Pool) == want

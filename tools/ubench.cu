@@ -1,5 +1,5 @@
-// developer micro-benchmarks (B200): fp64 latency / throughput, DSETP vs integer compares, smem
-// latency, ballot.  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench ubench.cu
+// developer micro-benchmarks (H100): fp64 latency / throughput, DSETP vs integer compares, smem
+// latency, ballot.  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench ubench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

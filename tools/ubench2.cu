@@ -1,5 +1,5 @@
 // developer micro-benchmark of the resolver's inner loop (one warp, lane = bin, D = 4):
-// cycles per entry for several formulations.  nvcc -gencode arch=compute_100a,code=sm_100a -O3
+// cycles per entry for several formulations.  nvcc -gencode arch=compute_90a,code=sm_90a -O3
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

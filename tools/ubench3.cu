@@ -1,7 +1,7 @@
 // developer micro-benchmark: the resolver's sequential loop, literal form versus the speculative form
 // (both outcomes of the next test are prepared off the critical chain; the chain is ballot -> select).
 // one CTA, nw warps each running its own copy; lane = bin (or node), D = 4.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o /tmp/ubench3 tools/ubench3.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o /tmp/ubench3 tools/ubench3.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
 // developer micro-benchmark: latency of the dependent steps a sequential placement loop is made of
 // (one warp, dependent chain of N iterations, cycles per iteration).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o build_tmp/ubench4 tools/ubench4.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o build_tmp/ubench4 tools/ubench4.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
 // developer micro-benchmark: throughput of the scan's inner loop (compare-only, thresholds in registers,
 // pod rows broadcast from shared memory) in DSETP per cycle per SM, for 8 and 16 warps per SM.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build_tmp/ubench5 tools/ubench5.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build_tmp/ubench5 tools/ubench5.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,7 +1,7 @@
-// ubench6.cu -- issue rate of the packed-rank scan's inner operation on sm_100a:
+// ubench6.cu -- issue rate of the packed-rank scan's inner operation on sm_90a:
 //     miss |= ((tg - r) & g) ^ g            (one IADD + one three-input LOP3 per packed word, acsfit_kernels.cuh)
 // measured as int32 lane-operations per clock and SM with every SM full of resident warps.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench6 tools/ubench6.cu && tools/ubench6
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench6 tools/ubench6.cu && tools/ubench6
 #include <cstdio>
 #include <cuda_runtime.h>
 

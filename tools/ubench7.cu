@@ -1,10 +1,10 @@
-// ubench7.cu -- cost of ONE placing step of the resolver, two formulations, on sm_100a:
+// ubench7.cu -- cost of ONE placing step of the resolver, two formulations, on sm_90a:
 //   vote:     lane = node, every lane tests the SAME entry, a ballot names the first fitting lane, that lane's state
 //             changes (the loop of firstfit_pipeline_kernel today);
 //   systolic: lane = node, lane i tests entry (step - i): the entry stream moves one lane per step, the only
 //             cross-lane traffic is the "still alive" bit (shfl_up), each lane's state recurrence is local.
 // Reports cycles per step for one active warp per CTA (the frontier is one warp) and for 8.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o tools/ubench7 tools/ubench7.cu && tools/ubench7
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o tools/ubench7 tools/ubench7.cu && tools/ubench7
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -179,7 +179,9 @@ void run(const char *name, int active_warps)
     long long *cyc;
     cudaMalloc(&rows, sizeof(double) * n * D);
     cudaMalloc(&out, 8);
-    cudaMalloc(&cyc, sizeof(long long) * 148 * 8);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&cyc, sizeof(long long) * sms * 8);
     cudaMemcpy(rows, h, sizeof(double) * n * D, cudaMemcpyHostToDevice);
     const size_t smem = ((size_t)n * D + 8 * 64 * D) * 8 + 8 * n;
     auto k = step_kernel<D, BINS, SYSTOLIC, INTCMP>;
@@ -188,7 +190,7 @@ void run(const char *name, int active_warps)
     unsigned ho[2];
     for (int rep = 0; rep < 2; ++rep) {
         cudaMemset(out, 0, 8);
-        k<<<148, 256, smem>>>(rows, n, active_warps, out, cyc);
+        k<<<sms, 256, smem>>>(rows, n, active_warps, out, cyc);
         cudaDeviceSynchronize();
     }
     cudaMemcpy(hc, cyc, sizeof(hc), cudaMemcpyDeviceToHost);
@@ -196,7 +198,7 @@ void run(const char *name, int active_warps)
     const int steps = SYSTOLIC ? (n / 32 + 1) * 32 : n;
     printf("%-28s D=%d warps=%d: %7lld cycles for %d entries = %6.1f cycles/entry (%d steps, %5.1f cycles/step), taken/warp %.1f  [%s]\n",
            name, D, active_warps, hc[0], n, (double)hc[0] / n, steps, (double)hc[0] / steps,
-           (double)ho[0] / (148.0 * active_warps), cudaGetErrorString(cudaGetLastError()));
+           (double)ho[0] / ((double)sms * active_warps), cudaGetErrorString(cudaGetLastError()));
     delete[] h;
 }
 
