@@ -107,7 +107,10 @@ ACSFIT_API acsfit_status acsfit_ctx_configure(acsfit_ctx *ctx, int min_stages, i
 /* the same developer knobs by name, after ctx creation: "ranks" (0: float64 compare scan, 1: packed-rank scan when
  * the tick's request table allows it -- the default), "stream" (1: the barrier-free streaming form of the pipeline
  * kernel, csrc/acsfit_stream_ff.cuh, where it applies; env ACSFIT_STREAM), "prune", "overlap", "min_stages", "inject_chain_timeout" (test hook), "cluster_blocks" (cluster
- * mode: cut the pod list of the node pass into this many blocks; 0 = automatic).  None changes a result. */
+ * mode: cut the pod list of the node pass into this many blocks; 0 = automatic).  None changes a result.
+ * Test hooks: "inject_chain_timeout" = n treats the next n chained node+bin launches as timed out (exercises the
+ * unchained redo); "bin_pass_stages" = n cuts every single-GPU bin pass, the chained first pass included, to at most
+ * n stages (0 = the library's limit of 1024), so that small inputs pack their bins in several passes. */
 ACSFIT_API acsfit_status acsfit_ctx_set_knob(acsfit_ctx *ctx, const char *name, int value);
 /* when enabled, the first-fit / bin-pack pipeline launches are bracketed with CUDA events on the
  * launching stream (read back with acsfit_last_pipeline_stats) */
@@ -307,6 +310,18 @@ ACSFIT_API uint64_t acsfit_launch_count(const acsfit_ctx *ctx);
  * decisions it evaluated, measured on the launching stream (bench.py roofline leg) */
 ACSFIT_API acsfit_status acsfit_last_pipeline_stats(const acsfit_ctx *ctx, double *out_ms,
                                          uint64_t *out_decisions, int *out_stages, int *out_tiles);
+
+/* test hook (read-only): the first-fit pipeline kernels the last API call on this ctx launched, in launch order,
+ * one record of ACSFIT_LAUNCH_FIELDS ints each, as launched (not as planned):
+ *   {pass (0 nodes, 1 bins), chained (1: node pass and first bin pass launched together on two streams), D,
+ *    RW (packed-rank words per row; 0 = float64 compare scan), prune (0/1), form (0 barrier, 1 streaming),
+ *    Tn (nodes / bins per stage), stages, resident (stage CTAs of this instantiation the GPU holds at once),
+ *    pool (visiting index; -1 for node passes), bin_base (first bin of the pass, clamped to INT32_MAX; -1 for
+ *    node passes), publish_every (barrier form: tiles between progress publications of an idle stage; 0 for the
+ *    streaming form)}
+ * At most max_records records are written to out; *out_n receives the number of records there are. */
+#define ACSFIT_LAUNCH_FIELDS 12
+ACSFIT_API acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, int max_records, int *out_n);
 
 /* developer probes (tools/perf_probe.py): per-stage clock64 phase totals [stages][8] of the last
  * pipeline launch (wait, load, scan, resolve, publish, refresh, hits, tiles) and a per-tile trace

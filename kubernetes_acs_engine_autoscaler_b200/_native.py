@@ -44,7 +44,12 @@ SIGNATURES = {
     "acsfit_debug_profile": (c_int, [c_vp, c_int, c_vp, c_int, c_vp]),
     "acsfit_debug_trace": (c_int, [c_vp, c_int, c_vp, c_int]),
     "acsfit_last_pipeline_stats": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "acsfit_last_launches": (c_int, [c_vp, c_vp, c_int, c_vp]),
 }
+
+# one record of acsfit_last_launches (ACSFIT_LAUNCH_FIELDS ints), field names in order
+LAUNCH_FIELDS = ("pass", "chained", "D", "RW", "prune", "form", "Tn", "stages", "resident", "pool", "bin_base",
+                 "publish_every")
 
 
 class AcsfitError(RuntimeError):

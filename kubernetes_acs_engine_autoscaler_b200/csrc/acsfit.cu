@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -46,7 +47,11 @@ struct acsfit_ctx {
     int epoch = 0;                                      // in-stream barrier count (same on every rank)
     int force_blocks = 0;                               // developer knob "cluster_blocks"
     int inject_chain_timeout = 0;                       // test knob: treat the next n chained launches as timed out
+    int bin_pass_stages = 0;                            // test knob: at most this many stages per bin pass (0: kMaxStagesPerPass)
     int chain_fallbacks = 0;                            // chained nodes+bins launches that hit the watchdog and were redone unchained
+    // launch records of the current API call (acsfit_last_launches); rec_* are set by the caller of a pipeline launch
+    std::vector<std::array<int, ACSFIT_LAUNCH_FIELDS>> launch_log;
+    int rec_chained = 0, rec_pool = -1;
     int cl_tn = 0, cl_stages = 0, cl_blocks = 0, cl_resident = 0;  // geometry of the last cluster node pass
     int smem_floor_kb = 0;    // >0: request at least this much dynamic smem per stage CTA (limits CTAs per SM)
     char err[512] = {0};
@@ -817,6 +822,7 @@ extern "C" acsfit_status acsfit_ctx_set_knob(acsfit_ctx *ctx, const char *name, 
     else if (!strcmp(name, "min_stages")) ctx->min_stages = std::max(0, value);
     else if (!strcmp(name, "cluster_blocks")) ctx->force_blocks = std::max(0, value);
     else if (!strcmp(name, "inject_chain_timeout")) ctx->inject_chain_timeout = std::max(0, value);
+    else if (!strcmp(name, "bin_pass_stages")) ctx->bin_pass_stages = std::max(0, value);
     else return fail(ctx, ACSFIT_E_INVALID, "unknown knob %s", name);
     return ACSFIT_OK;
 }
@@ -879,6 +885,15 @@ extern "C" acsfit_status acsfit_last_pipeline_stats(const acsfit_ctx *ctx, doubl
     return ACSFIT_OK;
 }
 
+extern "C" acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, int max_records, int *out_n)
+{
+    if (!ctx || !out_n || max_records < 0 || (max_records > 0 && !out)) return ACSFIT_E_INVALID;
+    const int n = (int)std::min<size_t>(ctx->launch_log.size(), (size_t)max_records);
+    for (int i = 0; i < n; ++i) memcpy(out + (size_t)i * ACSFIT_LAUNCH_FIELDS, ctx->launch_log[i].data(), sizeof(int) * ACSFIT_LAUNCH_FIELDS);
+    *out_n = (int)ctx->launch_log.size();
+    return ACSFIT_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // helpers shared by the entry points
 // ---------------------------------------------------------------------------------------------
@@ -892,6 +907,9 @@ static acsfit_status enter(acsfit_ctx *ctx, int D)
     if (e != cudaSuccess) return fail(ctx, ACSFIT_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(e));
     ctx->arena_off = 0;
     ctx->rk.nw = 0;  // rank tables live in the arena of one API call
+    ctx->launch_log.clear();
+    ctx->rec_chained = 0;
+    ctx->rec_pool = -1;
     return ACSFIT_OK;
 }
 
@@ -950,12 +968,10 @@ static acsfit_status build_ranks(acsfit_ctx *ctx, const double *req, int64_t row
     CUDA_TRY(cudaMemsetAsync(keys, 0xFF, sizeof(unsigned long long) * (size_t)D * kRankSlots, st));
     CUDA_TRY(cudaMemsetAsync(counts, 0, sizeof(int) * 16, st));
     rank_insert_kernel<<<grid_for(ctx, rows * D, 256), 256, 0, st>>>(req, rows, D, keys, counts);
-    static bool attr_set = false;
-    if (!attr_set) {
-        CUDA_TRY(cudaFuncSetAttribute(rank_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)(sizeof(unsigned long long) * kRankCap)));
-        attr_set = true;
-    }
+    // function attributes are per device: set at every call, like every other launch here, so that a ctx on a
+    // second device of the process gets the 64 KB too
+    CUDA_TRY(cudaFuncSetAttribute(rank_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)(sizeof(unsigned long long) * kRankCap)));
     rank_sort_kernel<<<D, 1024, sizeof(unsigned long long) * kRankCap, st>>>(keys, counts, sorted, ranks);
     ctx->launches += 2;
     int U[16];
@@ -1023,6 +1039,16 @@ static bool stream_form_ok(const acsfit_ctx *ctx, int D, int nw, int Tn)
     return ctx->use_stream && nw > 0 && D <= 8 && Tn >= 32 && Tn % 32 == 0;
 }
 
+// one acsfit_last_launches record, written by the two functions that launch a pipeline kernel, from the
+// instantiation they launch and the parameters it receives
+static void record_launch(acsfit_ctx *ctx, bool bins, int D, int rw, bool prune, bool streaming,
+                          const PipelineParams &q, int stages, int resident)
+{
+    ctx->launch_log.push_back({bins ? 1 : 0, ctx->rec_chained, D, rw, prune ? 1 : 0, streaming ? 1 : 0, q.Tn, stages,
+                               resident, bins ? ctx->rec_pool : -1,
+                               bins ? (int)std::min<int64_t>(q.bin_base, INT32_MAX) : -1, streaming ? 0 : q.publish_every});
+}
+
 template <int D, bool BINS, int RW>
 static acsfit_status launch_stream(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
@@ -1040,10 +1066,13 @@ static acsfit_status launch_stream(acsfit_ctx *ctx, const PipelineParams &pp, in
         *resident = it->second;
         return ACSFIT_OK;
     }
+    int held = 0;
+    TRY((launch_stream<D, BINS, RW>(ctx, pp, stages, st, &held)));
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<stages, 256, smem, st>>>(pp);
     ++ctx->launches;
     CUDA_TRY(cudaGetLastError());
+    record_launch(ctx, BINS, D, RW, false, true, pp, stages, held);
     return ACSFIT_OK;
 }
 
@@ -1076,11 +1105,10 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     }
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     PipelineParams q = pp;
-    {   // more stages than the GPU holds at once: several waves, each streaming the whole pod list (see the kernel's publish)
-        int held = 0;
-        TRY((launch_pipeline_w<D, BINS, PRUNE, RW>(ctx, pp, stages, st, &held)));
-        q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
-    }
+    // more stages than the GPU holds at once: several waves, each streaming the whole pod list (see the kernel's publish)
+    int held = 0;
+    TRY((launch_pipeline_w<D, BINS, PRUNE, RW>(ctx, pp, stages, st, &held)));
+    q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
     q.prof = (ctx->prof_dev && stages <= kProfStages) ? ctx->prof_dev : nullptr;
     if (q.prof) {
         CUDA_TRY(cudaMemsetAsync(ctx->prof_dev, 0, sizeof(unsigned long long) * (kProfStages + kProfTiles) * 8, st));
@@ -1091,6 +1119,7 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     kern<<<stages, NT, smem, st>>>(q);
     ++ctx->launches;
     CUDA_TRY(cudaGetLastError());
+    record_launch(ctx, BINS, D, RW, PRUNE, false, q, stages, held);
     return ACSFIT_OK;
 }
 
@@ -1626,6 +1655,12 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
 // ---------------------------------------------------------------------------------------------
 constexpr int kMaxStagesPerPass = 1024;
 
+// stages of one single-GPU bin pass at most (test knob "bin_pass_stages" lowers it; cluster mode plans its own)
+static int bin_pass_cap(const acsfit_ctx *ctx)
+{
+    return ctx->bin_pass_stages > 0 ? std::min(ctx->bin_pass_stages, kMaxStagesPerPass) : kMaxStagesPerPass;
+}
+
 static size_t fulfill_scratch(int64_t Pp, int T, int D)
 {
     const size_t nblocks = (size_t)((Pp + kCompactChunk - 1) / kCompactChunk) + 1;
@@ -1717,7 +1752,7 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
             }
             while (M > 0) {
                 const bool cl = ctx->world > 1;
-                StagePlan plan = plan_stages(ctx, M, kMaxStagesPerPass, D, true);  // at most one bin per pod
+                StagePlan plan = plan_stages(ctx, M, bin_pass_cap(ctx), D, true);  // at most one bin per pod
                 int64_t pass_bins = (int64_t)plan.stages * plan.Tn;
                 int *sy = sync_words;
                 uint32_t *al = alive;
@@ -1777,6 +1812,7 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                 pp.watchdog_ns = (unsigned long long)ctx->watchdog_ms * 1000000ull;
                 pp.rk = ctx->rk;
                 if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
+                ctx->rec_pool = t;
                 TRY(launch_pipeline<true>(ctx, D, pp, plan.stages, st));
                 if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev1, st));
                 if (cl) TRY(cluster_merge_placed(ctx, M, placed, st));  // every rank: the pass's complete placements
@@ -2082,12 +2118,12 @@ static int chained_capacity(acsfit_ctx *ctx, int D, int Tn_nodes, int Tn_bins)
 static acsfit_status first_fit_chained(acsfit_ctx *ctx, const double *req, const int32_t *list_f, int64_t F, int D,
                                        const double *cap_type, const int32_t *node_type, double *used, int64_t N,
                                        int32_t *placed_f, unsigned long long *decisions_dev,
-                                       const double *unit_row_dev, int32_t *bins_f, int64_t *bins_covered,
+                                       int pool, const double *unit_row_dev, int32_t *bins_f, int64_t *bins_covered,
                                        uint64_t *bin_evals, bool *did, cudaStream_t st)
 {
     *did = false;
     const StagePlan pn = plan_stages(ctx, N, 0, D, false);
-    StagePlan pb = plan_stages(ctx, F, kMaxStagesPerPass, D, true);
+    StagePlan pb = plan_stages(ctx, F, bin_pass_cap(ctx), D, true);
     // every stage CTA of both pipelines must be resident at the same time: the bins stages spin on the node
     // stages' counters, and the two grids are dispatched in no particular order
     const int room = chained_capacity(ctx, D, pn.Tn, pb.Tn) - pn.stages - 4;  // a little headroom
@@ -2149,9 +2185,12 @@ static acsfit_status first_fit_chained(acsfit_ctx *ctx, const double *req, const
 
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
     CUDA_TRY(cudaEventRecord(ctx->ev_fork, st));
+    ctx->rec_chained = 1;
+    ctx->rec_pool = pool;
     TRY(launch_pipeline<false>(ctx, D, a, pn.stages, st));        // nodes first: its CTAs are dispatched first
     CUDA_TRY(cudaStreamWaitEvent(ctx->side, ctx->ev_fork, 0));
     TRY(launch_pipeline<true>(ctx, D, b, pb.stages, ctx->side));
+    ctx->rec_chained = 0;
     CUDA_TRY(cudaEventRecord(ctx->ev_join, ctx->side));
     CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join, 0));
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev1, st));
@@ -2272,7 +2311,7 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
                 TAKE(used_backup, double, (size_t)N * D);
                 CUDA_TRY(cudaMemcpyAsync(used_backup, used, sizeof(double) * (size_t)N * D, cudaMemcpyDeviceToDevice, st));
                 acsfit_status cs = first_fit_chained(ctx, req, list_f, F, D, cap_type, node_type, used, N, placed_f, evals_dev + 1,
-                                                     unit_ord_dev + (size_t)t0 * D, bins_f, &covered, &bev, &chained, st);
+                                                     t0, unit_ord_dev + (size_t)t0 * D, bins_f, &covered, &bev, &chained, st);
                 if (cs == ACSFIT_OK && chained && ctx->inject_chain_timeout > 0) {  // test hook: exercise the recovery path
                     --ctx->inject_chain_timeout;
                     cs = ACSFIT_E_TIMEOUT;

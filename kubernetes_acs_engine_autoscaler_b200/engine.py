@@ -88,7 +88,8 @@ class Engine(object):
         self._check(self._lib.acsfit_ctx_set_timing(self._ctx, 1 if enabled else 0))
 
     def set_knob(self, name, value):
-        """developer knobs of include/acsfit.h ("ranks", "prune", "overlap", "min_stages", "cluster_blocks")."""
+        """developer knobs of include/acsfit.h ("ranks", "stream", "prune", "overlap", "min_stages", "cluster_blocks",
+        and the test hooks "inject_chain_timeout", "bin_pass_stages")."""
         self._check(self._lib.acsfit_ctx_set_knob(self._ctx, name.encode(), int(value)))
 
     def configure(self, min_stages=0, watchdog_ms=0):
@@ -136,6 +137,17 @@ class Engine(object):
         self._check(self._lib.acsfit_last_pipeline_stats(self._ctx, ctypes.byref(ms), ctypes.byref(dec),
                                                          ctypes.byref(stages), ctypes.byref(tiles)))
         return {"ms": ms.value, "decisions": dec.value, "stages": stages.value, "tiles": tiles.value}
+
+    def last_launches(self):
+        """test hook: the first-fit pipeline kernels the last call launched, one dict per launch in launch order
+        (keys: _native.LAUNCH_FIELDS; "pass" 0 = nodes / 1 = bins, "RW" 0 = float64 scan, "form" 1 = streaming)."""
+        nf = len(_native.LAUNCH_FIELDS)
+        n = ctypes.c_int(0)
+        self._check(self._lib.acsfit_last_launches(self._ctx, None, 0, ctypes.cast(ctypes.byref(n), ctypes.c_void_p)))
+        out = np.zeros((max(n.value, 1), nf), dtype=np.int32)
+        self._check(self._lib.acsfit_last_launches(self._ctx, _ptr(out), n.value,
+                                                   ctypes.cast(ctypes.byref(n), ctypes.c_void_p)))
+        return [dict(zip(_native.LAUNCH_FIELDS, (int(v) for v in row))) for row in out[:n.value]]
 
     def debug_profile(self, enabled=True):
         """developer probe: per-stage clock64 totals [stages, 8] of the last pipeline launch
