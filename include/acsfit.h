@@ -101,13 +101,19 @@ ACSFIT_API acsfit_status acsfit_ctx_destroy(acsfit_ctx *ctx);
  *                           (default: only when the pass has more stages than the GPU holds at once)
  *   ACSFIT_MIN_STAGES=n     same as acsfit_ctx_configure(min_stages) (default: one stage per SM)
  *   ACSFIT_SMEM_FLOOR_KB=n  request at least n KB of shared memory per stage CTA (limits CTAs per SM)
- *   ACSFIT_STREAM_BYTES=n   staging bytes per warp of the K1/K6 streaming kernels (2048 / 4096 / 8192)
+ *   ACSFIT_STREAM_BYTES=n   initial value of knob "stream_bytes" (below)
+ *   ACSFIT_BULK_CFG=n       initial value of knob "bulk_cfg" (below)
  *   ACSFIT_RANKS=0          never use the packed-rank scan (float64 compares instead; same results) */
 ACSFIT_API acsfit_status acsfit_ctx_configure(acsfit_ctx *ctx, int min_stages, int watchdog_ms);
 /* the same developer knobs by name, after ctx creation: "ranks" (0: float64 compare scan, 1: packed-rank scan when
  * the tick's request table allows it -- the default), "stream" (1: the barrier-free streaming form of the pipeline
  * kernel, csrc/acsfit_stream_ff.cuh, where it applies; env ACSFIT_STREAM), "prune", "overlap", "min_stages", "inject_chain_timeout" (test hook), "cluster_blocks" (cluster
- * mode: cut the pod list of the node pass into this many blocks; 0 = automatic).  None changes a result.
+ * mode: cut the pod list of the node pass into this many blocks; 0 = automatic), and for the K1 / K6 idle scan
+ * (csrc/acsfit_scan_plan.h): "bulk_cfg" (geometry of the bulk-copy form, contiguous tables, D <= 8:
+ * 0 = 8 KB x 8 warps, 1 = 16 KB x 12, 2 = 16 KB x 8, 3 = 32 KB x 6, anything else = 8 KB x 16, the default 4;
+ * D = 16 always uses 16 KB x 8) and "stream_bytes" (staging bytes per warp of the gather form, tables with
+ * run_idx: the smallest of 2048 (D <= 4) / 4096 (D <= 8) / 8192 that is >= the value; default 8192).
+ * Both are per ctx.  None changes a result.
  * Test hooks: "inject_chain_timeout" = n treats the next n chained node+bin launches as timed out (exercises the
  * unchained redo); "bin_pass_stages" = n cuts every single-GPU bin pass, the chained first pass included, to at most
  * n stages (0 = the library's limit of 1024), so that small inputs pack their bins in several passes. */
@@ -138,6 +144,10 @@ ACSFIT_API acsfit_status acsfit_feasible_mask(acsfit_ctx *ctx, const double *req
  *   run_idx may be NULL (here, in acsfit_node_states and in the *_host forms): the table is then CONTIGUOUS, the
  *   pods of node n are rows row_ptr[n] .. row_ptr[n+1] of req_run / flags_run.  That is the layout the host
  *   layer produces, and it lets K1 / K6 stream the table with bulk copies (csrc/acsfit_stream.cuh).
+ *   Alignment (here and in acsfit_node_states): the streaming forms for D in {2,4,8,16} read req_run -- and, for
+ *   a contiguous table in K6, flags_run -- with 16-byte copies, so they run only when those pointers are 16-byte
+ *   aligned.  Any other table (a view at an odd offset, e.g. flags[1:]) runs the per-thread form with scalar
+ *   loads: the same result, only slower.  acsfit_last_scan_launch reports which form ran.
  */
 ACSFIT_API acsfit_status acsfit_occupancy(acsfit_ctx *ctx, const int64_t *row_ptr, const int32_t *run_idx,
                                const double *req_run, int64_t N, int D, double *used_inout,
@@ -148,7 +158,9 @@ ACSFIT_API acsfit_status acsfit_occupancy(acsfit_ctx *ctx, const int64_t *row_pt
  * KubeNode.can_fit (kube.py:173-176): sequential first-fit of pods (list order) over nodes
  * (list order); a hit mutates used[node] += req.  Exact and order-preserving.
  *   req        [dev] req_rows x D     (D must be 2, 4, 8 or 16: zero columns are neutral, because
- *                                      an absent resource key is 0.0 on both sides of the test)
+ *                                      an absent resource key is 0.0 on both sides of the test;
+ *                                      16-byte aligned, else ACSFIT_E_INVALID -- the same holds for req
+ *                                      of acsfit_fulfill_pending and acsfit_scale_up)
  *   pod_idx    [dev] P int32 row numbers into req, the pods to schedule in order; NULL = rows 0..P-1
  *   cap_type   [dev] K x D, node_type [dev] N int32 (row of cap_type per node)
  *   used_inout [dev] N x D
@@ -322,6 +334,14 @@ ACSFIT_API acsfit_status acsfit_last_pipeline_stats(const acsfit_ctx *ctx, doubl
  * At most max_records records are written to out; *out_n receives the number of records there are. */
 #define ACSFIT_LAUNCH_FIELDS 12
 ACSFIT_API acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, int max_records, int *out_n);
+
+/* test hook (read-only): the K1 (occupancy) / K6 (node states) kernel the last API call on this ctx launched, as
+ * launched, one record of ACSFIT_SCAN_FIELDS ints written to out:
+ *   {kernel (0 none, 1 occupancy, 2 node states), form (0 per thread, 1 index gather, 2 bulk copy), D,
+ *    staging bytes per warp (0 per thread), warps per CTA, table entries per staging chunk (0 per thread),
+ *    grid (CTAs), S (idle thresholds; 0 for occupancy)} */
+#define ACSFIT_SCAN_FIELDS 8
+ACSFIT_API acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out);
 
 /* developer probes (tools/perf_probe.py): per-stage clock64 phase totals [stages][8] of the last
  * pipeline launch (wait, load, scan, resolve, publish, refresh, hits, tiles) and a per-tile trace

@@ -45,11 +45,14 @@ SIGNATURES = {
     "acsfit_debug_trace": (c_int, [c_vp, c_int, c_vp, c_int]),
     "acsfit_last_pipeline_stats": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "acsfit_last_launches": (c_int, [c_vp, c_vp, c_int, c_vp]),
+    "acsfit_last_scan_launch": (c_int, [c_vp, c_vp]),
 }
 
 # one record of acsfit_last_launches (ACSFIT_LAUNCH_FIELDS ints), field names in order
 LAUNCH_FIELDS = ("pass", "chained", "D", "RW", "prune", "form", "Tn", "stages", "resident", "pool", "bin_base",
                  "publish_every")
+# the record of acsfit_last_scan_launch (ACSFIT_SCAN_FIELDS ints), field names in order
+SCAN_FIELDS = ("kernel", "form", "D", "bytes", "warps", "chunk", "grid", "S")
 
 
 class AcsfitError(RuntimeError):

@@ -52,6 +52,9 @@ struct acsfit_ctx {
     // launch records of the current API call (acsfit_last_launches); rec_* are set by the caller of a pipeline launch
     std::vector<std::array<int, ACSFIT_LAUNCH_FIELDS>> launch_log;
     int rec_chained = 0, rec_pool = -1;
+    ScanLaunch scan_rec = {};  // the K1 / K6 kernel of the current API call (acsfit_last_scan_launch); kernel 0 = none
+    int bulk_cfg = 4;          // geometry of the K1 / K6 bulk-copy form (knob "bulk_cfg", env ACSFIT_BULK_CFG)
+    int stream_bytes = 8192;   // staging bytes per warp of the K1 / K6 gather form (knob "stream_bytes", env ACSFIT_STREAM_BYTES)
     int cl_tn = 0, cl_stages = 0, cl_blocks = 0, cl_resident = 0;  // geometry of the last cluster node pass
     int smem_floor_kb = 0;    // >0: request at least this much dynamic smem per stage CTA (limits CTAs per SM)
     char err[512] = {0};
@@ -397,10 +400,8 @@ __global__ void node_states_kernel(const int64_t *__restrict__ row_ptr, const in
 // vector loads, consecutive lanes -> consecutive CSR entries), then every lane consumes its own node's
 // entries in order.  The ordered left-to-right float64 sum of the reference is preserved; only the memory
 // access pattern changes (coalesced streaming instead of one scattered row per thread).
-constexpr int kStreamWarps = 8;
+// kStreamWarps warps per CTA (acsfit_scan_plan.h, where the staging bytes per warp are chosen).
 static int g_trace = 0;           // ACSFIT_TRACE=1: per-pass timings on stderr (with acsfit_ctx_set_timing)
-static int g_bulk_cfg = 4;        // geometry of the bulk-copy form (developer knob ACSFIT_BULK_CFG)
-static int g_stream_bytes = 8192;  // staging bytes per warp (developer knob ACSFIT_STREAM_BYTES: 2048 / 4096 / 8192)
 
 template <int D, bool STATES, int kStreamBytesPerWarp>
 __global__ void __launch_bounds__(kStreamWarps * 32)
@@ -587,7 +588,7 @@ static cudaError_t launch_node_stream_b(int grid, cudaStream_t st, const int64_t
                                       const double *req_run, const uint8_t *flags_run, const double *cap_type,
                                       const int32_t *node_type, const uint8_t *node_flags, const int64_t *node_age,
                                       int64_t N, int any_pending, const int64_t *thr, int S, uint8_t *out_state,
-                                      double *used)
+                                      double *used, ScanLaunch *rec)
 {
     constexpr int kChunk = kStreamBytesPerWarp / 2 / (8 * D);
     const size_t smem = (size_t)kStreamWarps * kStreamBytesPerWarp + (size_t)kStreamWarps * 2 * kChunk;
@@ -601,35 +602,34 @@ static cudaError_t launch_node_stream_b(int grid, cudaStream_t st, const int64_t
         grid = std::min(grid, per_sm * sms);
     kern<<<grid, kStreamWarps * 32, smem, st>>>(row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags,
                                                 node_age, N, any_pending, thr, S, out_state, used);
+    *rec = {STATES ? 2 : 1, kScanGather, D, kStreamBytesPerWarp, kStreamWarps, kChunk, grid, S};
     return cudaGetLastError();
 }
 
+// the bulk-copy or gather instantiation plan_scan chose (p.form is kScanBulk or kScanGather)
 template <int D, bool STATES>
-static cudaError_t launch_node_stream(int grid, cudaStream_t st, const int64_t *row_ptr, const int32_t *run_idx,
-                                      const double *req_run, const uint8_t *flags_run, const double *cap_type,
-                                      const int32_t *node_type, const uint8_t *node_flags, const int64_t *node_age,
-                                      int64_t N, int any_pending, const int64_t *thr, int S, uint8_t *out_state,
-                                      double *used)
+static cudaError_t launch_node_stream(const ScanPlan &p, int grid, cudaStream_t st, const int64_t *row_ptr,
+                                      const int32_t *run_idx, const double *req_run, const uint8_t *flags_run,
+                                      const double *cap_type, const int32_t *node_type, const uint8_t *node_flags,
+                                      const int64_t *node_age, int64_t N, int any_pending, const int64_t *thr, int S,
+                                      uint8_t *out_state, double *used, ScanLaunch *rec)
 {
-    if (!run_idx) {  // contiguous table: TMA bulk copies (acsfit_stream.cuh); geometry = <bytes per warp, warps>
-#define ACSFIT_BULK_ARGS grid, st, row_ptr, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr, S, out_state, used
+    if (p.form == kScanBulk) {  // contiguous table: TMA bulk copies (acsfit_stream.cuh); geometry = <bytes per warp, warps>
+#define ACSFIT_BULK_ARGS grid, st, row_ptr, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr, S, out_state, used, rec
         if constexpr (D <= 8) {
-            switch (g_bulk_cfg) {
-            case 1: return launch_node_stream_bulk<D, STATES, 16384, 12>(ACSFIT_BULK_ARGS);
-            case 2: return launch_node_stream_bulk<D, STATES, 16384, 8>(ACSFIT_BULK_ARGS);
-            case 3: return launch_node_stream_bulk<D, STATES, 32768, 6>(ACSFIT_BULK_ARGS);
-            case 4: return launch_node_stream_bulk<D, STATES, 8192, 16>(ACSFIT_BULK_ARGS);
-            case 0: return launch_node_stream_bulk<D, STATES, 8192, 8>(ACSFIT_BULK_ARGS);
-            default: return launch_node_stream_bulk<D, STATES, 8192, 16>(ACSFIT_BULK_ARGS);  // measured best on H100 (DESIGN.md section 6)
-            }
+            if (p.bytes_per_warp == 8192 && p.warps == 8) return launch_node_stream_bulk<D, STATES, 8192, 8>(ACSFIT_BULK_ARGS);
+            if (p.bytes_per_warp == 16384 && p.warps == 12) return launch_node_stream_bulk<D, STATES, 16384, 12>(ACSFIT_BULK_ARGS);
+            if (p.bytes_per_warp == 16384 && p.warps == 8) return launch_node_stream_bulk<D, STATES, 16384, 8>(ACSFIT_BULK_ARGS);
+            if (p.bytes_per_warp == 32768 && p.warps == 6) return launch_node_stream_bulk<D, STATES, 32768, 6>(ACSFIT_BULK_ARGS);
+            return launch_node_stream_bulk<D, STATES, 8192, 16>(ACSFIT_BULK_ARGS);  // measured best on H100 (DESIGN.md section 6)
         } else {
             return launch_node_stream_bulk<D, STATES, 16384, 8>(ACSFIT_BULK_ARGS);
         }
 #undef ACSFIT_BULK_ARGS
     }
-#define ACSFIT_STREAM_ARGS grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr, S, out_state, used
-    if constexpr (D <= 4) { if (g_stream_bytes <= 2048) return launch_node_stream_b<D, STATES, 2048>(ACSFIT_STREAM_ARGS); }
-    if constexpr (D <= 8) { if (g_stream_bytes <= 4096) return launch_node_stream_b<D, STATES, 4096>(ACSFIT_STREAM_ARGS); }
+#define ACSFIT_STREAM_ARGS grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr, S, out_state, used, rec
+    if constexpr (D <= 4) { if (p.bytes_per_warp == 2048) return launch_node_stream_b<D, STATES, 2048>(ACSFIT_STREAM_ARGS); }
+    if constexpr (D <= 8) { if (p.bytes_per_warp == 4096) return launch_node_stream_b<D, STATES, 4096>(ACSFIT_STREAM_ARGS); }
     return launch_node_stream_b<D, STATES, 8192>(ACSFIT_STREAM_ARGS);
 #undef ACSFIT_STREAM_ARGS
 }
@@ -772,8 +772,8 @@ extern "C" acsfit_status acsfit_ctx_create(int device, acsfit_ctx **out_ctx)
     if (const char *env = getenv("ACSFIT_STREAM")) ctx->use_stream = atoi(env) != 0;
     memset(&ctx->rk, 0, sizeof ctx->rk);
     if (const char *env = getenv("ACSFIT_MIN_STAGES")) ctx->min_stages = std::max(0, atoi(env));
-    if (const char *env = getenv("ACSFIT_STREAM_BYTES")) g_stream_bytes = atoi(env);
-    if (const char *env = getenv("ACSFIT_BULK_CFG")) g_bulk_cfg = atoi(env);
+    if (const char *env = getenv("ACSFIT_STREAM_BYTES")) ctx->stream_bytes = atoi(env);
+    if (const char *env = getenv("ACSFIT_BULK_CFG")) ctx->bulk_cfg = atoi(env);
     if (const char *env = getenv("ACSFIT_TRACE")) g_trace = atoi(env);
     if (cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
@@ -823,6 +823,8 @@ extern "C" acsfit_status acsfit_ctx_set_knob(acsfit_ctx *ctx, const char *name, 
     else if (!strcmp(name, "cluster_blocks")) ctx->force_blocks = std::max(0, value);
     else if (!strcmp(name, "inject_chain_timeout")) ctx->inject_chain_timeout = std::max(0, value);
     else if (!strcmp(name, "bin_pass_stages")) ctx->bin_pass_stages = std::max(0, value);
+    else if (!strcmp(name, "bulk_cfg")) ctx->bulk_cfg = value;
+    else if (!strcmp(name, "stream_bytes")) ctx->stream_bytes = value;
     else return fail(ctx, ACSFIT_E_INVALID, "unknown knob %s", name);
     return ACSFIT_OK;
 }
@@ -894,10 +896,26 @@ extern "C" acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, i
     return ACSFIT_OK;
 }
 
+extern "C" acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out)
+{
+    static_assert(sizeof(ScanLaunch) == sizeof(int) * ACSFIT_SCAN_FIELDS, "one int per record field");
+    if (!ctx || !out) return ACSFIT_E_INVALID;
+    memcpy(out, &ctx->scan_rec, sizeof(ScanLaunch));
+    return ACSFIT_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // helpers shared by the entry points
 // ---------------------------------------------------------------------------------------------
 static bool pipeline_dims_ok(int D) { return D == 2 || D == 4 || D == 8 || D == 16; }
+
+// the first-fit pipeline reads request rows as 16-byte double2 vectors (load_row / prefetch_row); there is no
+// scalar fall-back, so a table that is not 16-byte aligned is refused before anything is launched
+static acsfit_status check_req_aligned(acsfit_ctx *ctx, const double *req, const char *what)
+{
+    if (!aligned16(req)) return fail(ctx, ACSFIT_E_INVALID, "%s: req must be 16-byte aligned", what);
+    return ACSFIT_OK;
+}
 
 static acsfit_status enter(acsfit_ctx *ctx, int D)
 {
@@ -908,6 +926,7 @@ static acsfit_status enter(acsfit_ctx *ctx, int D)
     ctx->arena_off = 0;
     ctx->rk.nw = 0;  // rank tables live in the arena of one API call
     ctx->launch_log.clear();
+    ctx->scan_rec = ScanLaunch{};
     ctx->rec_chained = 0;
     ctx->rec_pool = -1;
     return ACSFIT_OK;
@@ -1880,30 +1899,40 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
     return ACSFIT_OK;
 }
 
-// K6 dispatch: the streaming form for padded column counts, the simple per-thread form otherwise
+// upper bound of the streaming forms' grid (they shrink it to the CTAs the GPU holds at once)
+static int stream_grid(const acsfit_ctx *ctx, int64_t N)
+{
+    return (int)std::max<int64_t>(1, std::min<int64_t>(((N + 31) / 32 + kStreamWarps - 1) / kStreamWarps,
+                                                       (int64_t)ctx->num_sms * 16));
+}
+
+// K6 dispatch: the form plan_scan picks (acsfit_scan_plan.h) -- a streaming form for padded column counts and
+// 16-byte aligned tables, the simple per-thread form otherwise
 static acsfit_status run_node_states(acsfit_ctx *ctx, const int64_t *row_ptr, const int32_t *run_idx,
                                      const double *req_run, const uint8_t *flags_run, const double *cap_type,
                                      const int32_t *node_type, const uint8_t *node_flags, const int64_t *node_age,
                                      int64_t N, int D, int any_pending, const int64_t *thr_dev, int S,
                                      uint8_t *out_state, cudaStream_t st)
 {
-    if (D == 2 || D == 4 || D == 8 || D == 16) {
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(((N + 31) / 32 + kStreamWarps - 1) / kStreamWarps,
-                                                                      (int64_t)ctx->num_sms * 16));
+    const ScanPlan p = plan_scan(D, true, run_idx, req_run, flags_run, ctx->bulk_cfg, ctx->stream_bytes);
+    ScanLaunch *rec = &ctx->scan_rec;
+    if (p.form != kScanPerThread) {
+        const int grid = stream_grid(ctx, N);
         cudaError_t e;
         switch (D) {
-        case 2: e = launch_node_stream<2, true>(grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr); break;
-        case 4: e = launch_node_stream<4, true>(grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr); break;
-        case 8: e = launch_node_stream<8, true>(grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr); break;
-        default: e = launch_node_stream<16, true>(grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr); break;
+        case 2: e = launch_node_stream<2, true>(p, grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr, rec); break;
+        case 4: e = launch_node_stream<4, true>(p, grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr, rec); break;
+        case 8: e = launch_node_stream<8, true>(p, grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr, rec); break;
+        default: e = launch_node_stream<16, true>(p, grid, st, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, any_pending, thr_dev, S, out_state, nullptr, rec); break;
         }
         ++ctx->launches;
         if (e != cudaSuccess) return fail(ctx, ACSFIT_E_CUDA, "node_states: %s", cudaGetErrorString(e));
         return ACSFIT_OK;
     }
-    node_states_kernel<<<grid_for(ctx, N, 128), 128, 0, st>>>(row_ptr, run_idx, req_run, flags_run, cap_type, node_type,
-                                                             node_flags, node_age, N, D, any_pending, thr_dev, S,
-                                                             out_state);
+    const int grid = grid_for(ctx, N, kPerThreadBlock);
+    node_states_kernel<<<grid, kPerThreadBlock, 0, st>>>(row_ptr, run_idx, req_run, flags_run, cap_type, node_type,
+                                                         node_flags, node_age, N, D, any_pending, thr_dev, S, out_state);
+    *rec = {2, kScanPerThread, D, 0, kPerThreadBlock / 32, 0, grid, S};
     ++ctx->launches;
     CUDA_TRY(cudaGetLastError());
     return ACSFIT_OK;
@@ -1938,21 +1967,24 @@ extern "C" acsfit_status acsfit_occupancy(acsfit_ctx *ctx, const int64_t *row_pt
     if (N < 0 || (N > 0 && (!row_ptr || !used_inout)))
         return fail(ctx, ACSFIT_E_INVALID, "occupancy: bad arguments");
     if (N == 0) return ACSFIT_OK;
-    if (D == 2 || D == 4 || D == 8 || D == 16) {
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(((N + 31) / 32 + kStreamWarps - 1) / kStreamWarps,
-                                                                      (int64_t)ctx->num_sms * 16));
+    const ScanPlan p = plan_scan(D, false, run_idx, req_run, nullptr, ctx->bulk_cfg, ctx->stream_bytes);
+    ScanLaunch *rec = &ctx->scan_rec;
+    if (p.form != kScanPerThread) {
+        const int grid = stream_grid(ctx, N);
         cudaError_t e;
         switch (D) {
-        case 2: e = launch_node_stream<2, false>(grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout); break;
-        case 4: e = launch_node_stream<4, false>(grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout); break;
-        case 8: e = launch_node_stream<8, false>(grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout); break;
-        default: e = launch_node_stream<16, false>(grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout); break;
+        case 2: e = launch_node_stream<2, false>(p, grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout, rec); break;
+        case 4: e = launch_node_stream<4, false>(p, grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout, rec); break;
+        case 8: e = launch_node_stream<8, false>(p, grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout, rec); break;
+        default: e = launch_node_stream<16, false>(p, grid, st, row_ptr, run_idx, req_run, nullptr, nullptr, nullptr, nullptr, nullptr, N, 0, nullptr, 0, nullptr, used_inout, rec); break;
         }
         ++ctx->launches;
         if (e != cudaSuccess) return fail(ctx, ACSFIT_E_CUDA, "occupancy: %s", cudaGetErrorString(e));
         return ACSFIT_OK;
     }
-    occupancy_kernel<<<grid_for(ctx, N, 128), 128, 0, st>>>(row_ptr, run_idx, req_run, N, D, used_inout);
+    const int grid = grid_for(ctx, N, kPerThreadBlock);
+    occupancy_kernel<<<grid, kPerThreadBlock, 0, st>>>(row_ptr, run_idx, req_run, N, D, used_inout);
+    *rec = {1, kScanPerThread, D, 0, kPerThreadBlock / 32, 0, grid, 0};
     ++ctx->launches;
     CUDA_TRY(cudaGetLastError());
     return ACSFIT_OK;
@@ -1971,6 +2003,7 @@ extern "C" acsfit_status acsfit_first_fit_nodes(acsfit_ctx *ctx, const double *r
         return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes: bad arguments");
     if (!pipeline_dims_ok(D))
         return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
+    TRY(check_req_aligned(ctx, req, "first_fit_nodes"));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + 1024, st));
     ctx->arena_off = 0;
@@ -2000,6 +2033,7 @@ extern "C" acsfit_status acsfit_fulfill_pending(acsfit_ctx *ctx, const double *r
         return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending: bad arguments");
     if (!pipeline_dims_ok(D))
         return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
+    TRY(check_req_aligned(ctx, req, "fulfill_pending"));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + 1024, st));
     ctx->arena_off = 0;
@@ -2405,6 +2439,7 @@ extern "C" acsfit_status acsfit_scale_up(acsfit_ctx *ctx, const double *req, int
     TRY(scale_up_check(ctx, req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T, cap_type,
                        node_type, used_inout, N, out_feasible, out_placed, out_new_size, out_units_needed,
                        out_bins_opened, out_acc_pool, out_counters));
+    TRY(check_req_aligned(ctx, req, "scale_up"));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, scale_up_scratch(ctx, P, N, T, D), st));
     ctx->arena_off = 0;

@@ -8,13 +8,16 @@
 //     completed on an mbarrier -- no per-lane address arithmetic, no index gather, no
 //     16-byte cp.async fan-out;
 //   * chunk boundaries are multiples of 16 entries from the start of the table, so every copy is 16-byte aligned
-//     in global and shared memory (the first chunk may start a few entries before the warp's range: ignored);
+//     in global and shared memory (the first chunk may start a few entries before the warp's range: ignored) --
+//     provided req_run and flags_run themselves are 16-byte aligned, which plan_scan (acsfit_scan_plan.h) checks
+//     before it picks this form;
 //   * the consume loop is branch-free: a pod that does not count (a mirrored pod in get_node_state) adds +0.0,
 //     which leaves a non-negative float64 sum bit-identical, so lanes never diverge on the flag test.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
 #include "../../include/acsfit.h"
+#include "acsfit_scan_plan.h"
 
 namespace acsfit {
 
@@ -222,7 +225,7 @@ template <int D, bool STATES, int kBytesPerWarp, int kBulkWarps>
 static cudaError_t launch_node_stream_bulk(int grid, cudaStream_t st, const int64_t *row_ptr, const double *req_run,
                                            const uint8_t *flags_run, const double *cap_type, const int32_t *node_type,
                                            const uint8_t *node_flags, const int64_t *node_age, int64_t N, int any_pending,
-                                           const int64_t *thr, int S, uint8_t *out_state, double *used)
+                                           const int64_t *thr, int S, uint8_t *out_state, double *used, ScanLaunch *rec)
 {
     constexpr int kChunk = kBytesPerWarp / 2 / (8 * D);
     const size_t smem = (size_t)kBulkWarps * kBytesPerWarp + (size_t)kBulkWarps * 2 * kChunk + (size_t)kBulkWarps * 2 * sizeof(uint64_t);
@@ -235,6 +238,7 @@ static cudaError_t launch_node_stream_bulk(int grid, cudaStream_t st, const int6
         grid = per_sm * sms;  // persistent: exactly the resident CTAs (each warp takes a contiguous range of groups)
     kern<<<grid, kBulkWarps * 32, smem, st>>>(row_ptr, req_run, flags_run, cap_type, node_type, node_flags, node_age, N,
                                               any_pending, thr, S, out_state, used);
+    *rec = {STATES ? 2 : 1, kScanBulk, D, kBytesPerWarp, kBulkWarps, kChunk, grid, S};
     return cudaGetLastError();
 }
 

@@ -89,7 +89,7 @@ class Engine(object):
 
     def set_knob(self, name, value):
         """developer knobs of include/acsfit.h ("ranks", "stream", "prune", "overlap", "min_stages", "cluster_blocks",
-        and the test hooks "inject_chain_timeout", "bin_pass_stages")."""
+        "bulk_cfg", "stream_bytes", and the test hooks "inject_chain_timeout", "bin_pass_stages")."""
         self._check(self._lib.acsfit_ctx_set_knob(self._ctx, name.encode(), int(value)))
 
     def configure(self, min_stages=0, watchdog_ms=0):
@@ -148,6 +148,13 @@ class Engine(object):
         self._check(self._lib.acsfit_last_launches(self._ctx, _ptr(out), n.value,
                                                    ctypes.cast(ctypes.byref(n), ctypes.c_void_p)))
         return [dict(zip(_native.LAUNCH_FIELDS, (int(v) for v in row))) for row in out[:n.value]]
+
+    def last_scan_launch(self):
+        """test hook: the K1 / K6 kernel the last call launched, as a dict (keys: _native.SCAN_FIELDS; "kernel"
+        0 = none / 1 = occupancy / 2 = node states, "form" 0 = per thread / 1 = index gather / 2 = bulk copy)."""
+        out = np.zeros(len(_native.SCAN_FIELDS), dtype=np.int32)
+        self._check(self._lib.acsfit_last_scan_launch(self._ctx, _ptr(out)))
+        return dict(zip(_native.SCAN_FIELDS, (int(v) for v in out)))
 
     def debug_profile(self, enabled=True):
         """developer probe: per-stage clock64 totals [stages, 8] of the last pipeline launch
