@@ -271,6 +271,78 @@ ACSFIT_API acsfit_status acsfit_scale_up_host(acsfit_ctx *ctx, const double *req
                                    int64_t *out_units_needed, int64_t *out_bins_opened,
                                    int32_t *out_acc_pool, uint64_t *out_counters);
 
+/*
+ * Node selectors (opt-in): the scale-up decision honours the pods' spec.nodeSelector, with the rules of the upstream
+ * ec2 autoscaler the reference descends from:
+ *   feasibility   a pod is schedulable when some agent pool (ignored pools included) matches its selector AND
+ *                 (unit - req).possible
+ *   first fit     the first node in list order with node.is_match(pod) and node.can_fit(pod.resources) takes it
+ *   bin packing   the pool gate of fulfill_pending is "pool matches AND (unit - req).possible"; bins, clamp
+ *                 arithmetic and accounting are unchanged (every new node of a pool carries the pool's labels)
+ *   counters      unchanged formulas: one evaluation per (pod, node) pair or (pod, pool) visited, one per gate
+ *                 and bin test (the match is evaluated first and short-circuits; it is not an extra evaluation)
+ * The host maps every distinct match signature (set of matching nodes, set of matching pools) to a class number
+ * < classes <= ACSFIT_MAX_CLASSES.  Class 0 = no selector: its bit must be set in every mask (checked: pool masks on
+ * the host, node masks on the device, ACSFIT_E_INVALID otherwise).  A pod may take a node / pool exactly when bit
+ * pod_class of that mask is set.
+ *   pod_class          [dev] one byte per row of req (indexed like req rows), each < classes (else ACSFIT_E_INVALID)
+ *   node_match         [dev] N masks
+ *   pool_match_all     [host] T masks in agent_pools order (feasibility)
+ *   pool_match_ordered [host] T masks in VISITING order (pool gate of fulfill_pending)
+ * In acsfit_scale_up_sel_host pod_class and node_match are host pointers too.  An entry point reads only the
+ * fields it needs.  Scope: the node pass with selectors runs the barrier form of the pipeline kernel only (it
+ * ignores the "stream" knob: acsfit_last_launches shows form 0), and cluster mode (world > 1) refuses the
+ * *_sel entry points with ACSFIT_E_INVALID.
+ */
+#define ACSFIT_MAX_CLASSES 64
+typedef struct acsfit_selectors {
+    const uint8_t *pod_class;
+    const uint64_t *node_match;
+    const uint64_t *pool_match_all;
+    const uint64_t *pool_match_ordered;
+    int classes;
+} acsfit_selectors;
+
+/* the selector forms of the entry points above: the same arguments plus `sel`, the same outputs */
+ACSFIT_API acsfit_status acsfit_feasible_mask_sel(acsfit_ctx *ctx, const double *req, int64_t P, int D,
+                                                  const double *unit, int T, const acsfit_selectors *sel,
+                                                  uint8_t *out_mask, uint64_t *out_evals, acsfit_stream_t stream);
+ACSFIT_API acsfit_status acsfit_first_fit_nodes_sel(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                    const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                    const int32_t *node_type, double *used_inout, int64_t N,
+                                                    const acsfit_selectors *sel, int32_t *out_placed,
+                                                    uint64_t *out_decisions, acsfit_stream_t stream);
+ACSFIT_API acsfit_status acsfit_fulfill_pending_sel(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                    int64_t num_listed, int D, const double *unit,
+                                                    const int32_t *pool_actual, const int32_t *pool_max,
+                                                    const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                    const acsfit_selectors *sel, int64_t *out_new_size,
+                                                    int64_t *out_units_needed, int64_t *out_bins_opened,
+                                                    int32_t *out_acc_pool, int32_t *out_bin_of,
+                                                    int64_t *out_unaccounted, uint64_t *out_evals,
+                                                    acsfit_stream_t stream);
+/* including the chained node + first-bin-pass launch (when every pod to schedule is eligible for the first pool
+ * visited, match included) and its watchdog redo */
+ACSFIT_API acsfit_status acsfit_scale_up_sel(acsfit_ctx *ctx, const double *req, int64_t P, int D,
+                                             const double *unit_all, const double *unit_ordered,
+                                             const int32_t *pool_actual, const int32_t *pool_max,
+                                             const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                             const double *cap_type, const int32_t *node_type, double *used_inout,
+                                             int64_t N, const acsfit_selectors *sel, uint8_t *out_feasible,
+                                             int32_t *out_placed, int64_t *out_new_size, int64_t *out_units_needed,
+                                             int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                             uint64_t *out_counters, acsfit_stream_t stream);
+ACSFIT_API acsfit_status acsfit_scale_up_sel_host(acsfit_ctx *ctx, const double *req, int64_t P, int D,
+                                                  const double *unit_all, const double *unit_ordered,
+                                                  const int32_t *pool_actual, const int32_t *pool_max,
+                                                  const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                  const double *cap_type, int K, const int32_t *node_type,
+                                                  double *used_inout, int64_t N, const acsfit_selectors *sel,
+                                                  uint8_t *out_feasible, int32_t *out_placed,
+                                                  int64_t *out_new_size, int64_t *out_units_needed,
+                                                  int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                                  uint64_t *out_counters);
+
 /* acsfit_occupancy_host = acsfit_occupancy with host buffers (reference cluster.py:165-168): R rows of req_run,
  * used_inout N x D is read, updated and written back. */
 ACSFIT_API acsfit_status acsfit_occupancy_host(acsfit_ctx *ctx, const int64_t *row_ptr, const int32_t *run_idx,
@@ -342,6 +414,11 @@ ACSFIT_API acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, i
  *    grid (CTAs), S (idle thresholds; 0 for occupancy)} */
 #define ACSFIT_SCAN_FIELDS 8
 ACSFIT_API acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out);
+
+/* test hook (read-only): the pods the candidate scan of the last call's selector node passes handed to the resolver,
+ * summed over tiles and stages (a pod counts once per stage in which some node fits it AND matches its class); 0 after a
+ * call without a selector node pass */
+ACSFIT_API acsfit_status acsfit_last_sel_hits(const acsfit_ctx *ctx, uint64_t *out);
 
 /* developer probes (tools/perf_probe.py): per-stage clock64 phase totals [stages][8] of the last
  * pipeline launch (wait, load, scan, resolve, publish, refresh, hits, tiles) and a per-tile trace

@@ -46,7 +46,25 @@ SIGNATURES = {
     "acsfit_last_pipeline_stats": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "acsfit_last_launches": (c_int, [c_vp, c_vp, c_int, c_vp]),
     "acsfit_last_scan_launch": (c_int, [c_vp, c_vp]),
+    "acsfit_last_sel_hits": (c_int, [c_vp, c_vp]),
+    # node selectors: the arguments of the plain form plus a `const acsfit_selectors *` (Selectors below)
+    "acsfit_feasible_mask_sel": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "acsfit_first_fit_nodes_sel": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                                           c_vp, c_vp]),
+    "acsfit_fulfill_pending_sel": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
+                                           c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "acsfit_scale_up_sel": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
+                                    c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "acsfit_scale_up_sel_host": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
+                                         c_vp, c_int, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                         c_vp]),
 }
+
+
+class Selectors(ctypes.Structure):
+    """struct acsfit_selectors (include/acsfit.h)"""
+    _fields_ = [("pod_class", c_vp), ("node_match", c_vp), ("pool_match_all", c_vp),
+                ("pool_match_ordered", c_vp), ("classes", c_int)]
 
 # one record of acsfit_last_launches (ACSFIT_LAUNCH_FIELDS ints), field names in order
 LAUNCH_FIELDS = ("pass", "chained", "D", "RW", "prune", "form", "Tn", "stages", "resident", "pool", "bin_base",

@@ -5,6 +5,9 @@ from .capacity import get_capacity_for_instance_type
 
 logger = logging.getLogger('autoscaler.agent_pool')
 
+# labels of one node that a new node of the same pool does not inherit
+_NODE_ONLY_LABELS = ('kubernetes.io/hostname', 'openai/cordoned-by-autoscaler')
+
 
 class AgentPool(object):
     def __init__(self, pool_name, instance_type, nodes):
@@ -21,6 +24,25 @@ class AgentPool(object):
     @property
     def unit_capacity(self):
         return get_capacity_for_instance_type(self.instance_type)
+
+    @property
+    def labels(self):
+        """the labels a new node of this pool will carry, for matching node selectors: every label all current nodes
+        share with the same value, except the per-node hostname and the autoscaler's cordon mark, plus the pool name
+        and instance type, which are always set (an empty pool has just those two)."""
+        common = None
+        for node in self.nodes:
+            node_labels = node.selectors
+            if common is None:
+                common = dict(node_labels)
+            else:
+                common = {k: v for k, v in common.items() if k in node_labels and node_labels[k] == v}
+        common = common or {}
+        for key in _NODE_ONLY_LABELS:
+            common.pop(key, None)
+        common['agentpool'] = self.name
+        common['beta.kubernetes.io/instance-type'] = self.instance_type
+        return common
 
     def reclaim_unschedulable_nodes(self, new_desired_capacity):
         """uncordon just enough of our own cordoned nodes before asking for new VMs

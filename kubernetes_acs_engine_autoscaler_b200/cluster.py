@@ -54,8 +54,13 @@ class Cluster(object):
                  subscription_id, client_private_key, ca_private_key,
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
-                 over_provision=5, dry_run=False):
+                 over_provision=5, dry_run=False, node_selectors=None):
         self.kubeconfig = kubeconfig
+        # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
+        # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
+        if node_selectors is None:
+            node_selectors = os.environ.get('ACSFIT_NODE_SELECTORS', '0') not in ('', '0')
+        self.node_selectors = bool(node_selectors)
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -155,7 +160,7 @@ class Cluster(object):
             resource_group=self.resource_group, nodes=all_nodes, deployments=self.deployments,
             arm_template=self.arm_template, arm_parameters=self.arm_parameters, dry_run=self.dry_run,
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
-            idle_threshold=self.idle_threshold, notifier=self.notifier)
+            idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [
@@ -183,7 +188,8 @@ class Cluster(object):
         """sequential first fit of the pods over the nodes (cluster.py:184-204); placed pods are
         counted into node.used_capacity, the rest are returned in order."""
         pods, nodes = list(pods), list(nodes)
-        placed = snapshot.first_fit_nodes(pods, nodes)
+        classes = snapshot.selector_classes(pods, nodes, []) if self.node_selectors else None
+        placed = snapshot.first_fit_nodes(pods, nodes, classes=classes)
         detail = len(pods) <= LOG_DETAIL_LIMIT
         pending_pods = []
         for i, pod in enumerate(pods):
@@ -210,12 +216,24 @@ class Cluster(object):
         """pending, unassigned pods that fit an empty instance of at least one pool
         (cluster.py:217-240)."""
         pending_unassigned_pods = [p for p in pods if p.status == KubePodStatus.PENDING and (not p.node_name)]
-        feasible = snapshot.feasible_pods(pending_unassigned_pods, agent_pools)
+        classes = None
+        if self.node_selectors:
+            classes = snapshot.selector_classes(pending_unassigned_pods, [], agent_pools)
+        feasible = snapshot.feasible_pods(pending_unassigned_pods, agent_pools, classes=classes)
+        unmatched = set()  # rejected only because no pool that would fit matches the node selector
+        if classes is not None and not classes.trivial:
+            rejected = [p for p, ok, c in zip(pending_unassigned_pods, feasible, classes.pod_class) if not ok and c]
+            if rejected:
+                fits = snapshot.feasible_pods(rejected, agent_pools)
+                unmatched = {id(p) for p, ok in zip(rejected, fits) if ok}
         pods_to_schedule = []
         warn = logger.isEnabledFor(logging.WARNING)  # (the message is formatted eagerly, as upstream: skip it when nobody listens)
         for pod, ok in zip(pending_unassigned_pods, feasible):
             if ok:
                 pods_to_schedule.append(pod)
+            elif warn and id(pod) in unmatched:
+                logger.warning("Pending pod %s cannot fit: no agent pool matches its node selector %s. "
+                               "Scheduling skipped." % (pod.name, pod.selectors))
             elif warn:
                 logger.warning("Pending pod %s cannot fit. "
                             "Please check that requested resource amount is "

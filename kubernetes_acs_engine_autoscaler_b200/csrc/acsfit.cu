@@ -49,6 +49,7 @@ struct acsfit_ctx {
     int inject_chain_timeout = 0;                       // test knob: treat the next n chained launches as timed out
     int bin_pass_stages = 0;                            // test knob: at most this many stages per bin pass (0: kMaxStagesPerPass)
     int chain_fallbacks = 0;                            // chained nodes+bins launches that hit the watchdog and were redone unchained
+    uint64_t last_sel_hits = 0;                         // hit entries of the selector node passes of the last call (acsfit_last_sel_hits)
     // launch records of the current API call (acsfit_last_launches); rec_* are set by the caller of a pipeline launch
     std::vector<std::array<int, ACSFIT_LAUNCH_FIELDS>> launch_log;
     int rec_chained = 0, rec_pool = -1;
@@ -322,6 +323,37 @@ __global__ void count_ineligible_kernel(const uint8_t *feasible, const double *r
         }
     for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xFFFFFFFFu, c, o);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
+}
+// the same with node selectors: a feasible pod is ineligible when the pool does not match its class either
+__global__ void count_ineligible_sel_kernel(const uint8_t *feasible, const double *req, int64_t P, int D,
+                                            const double *unit, unsigned long long pool_match, const uint8_t *pod_class,
+                                            unsigned long long *out)
+{
+    unsigned long long c = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < P; i += (int64_t)gridDim.x * blockDim.x)
+        if (feasible[i]) {
+            bool all = ((pool_match >> pod_class[i]) & 1ull) != 0ull;
+            for (int d = 0; d < D; ++d) all = all && fits_bin(unit[d], req[(size_t)i * D + d]);
+            c += all ? 0 : 1;
+        }
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xFFFFFFFFu, c, o);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
+}
+// selector classes must be < classes (<= 64): the kernels shift a 64-bit mask by the class; flag[0] |= 1 otherwise
+// class 0 (no selector) matches every node: bit 0 of every node mask must be set; flag[0] |= 2 otherwise
+__global__ void node_mask_check_kernel(const unsigned long long *node_match, int64_t n, int *flag)
+{
+    int bad = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        bad |= !(node_match[i] & 1ull);
+    if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 2);
+}
+__global__ void class_check_kernel(const uint8_t *pod_class, int64_t n, int classes, int *flag)
+{
+    int bad = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        bad |= pod_class[i] >= classes;
+    if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 1);
 }
 
 // scaler.py:172-175: pods of the first `take` bins become accounted
@@ -896,6 +928,13 @@ extern "C" acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, i
     return ACSFIT_OK;
 }
 
+extern "C" acsfit_status acsfit_last_sel_hits(const acsfit_ctx *ctx, uint64_t *out)
+{
+    if (!ctx || !out) return ACSFIT_E_INVALID;
+    *out = ctx->last_sel_hits;
+    return ACSFIT_OK;
+}
+
 extern "C" acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out)
 {
     static_assert(sizeof(ScanLaunch) == sizeof(int) * ACSFIT_SCAN_FIELDS, "one int per record field");
@@ -1096,22 +1135,23 @@ static acsfit_status launch_stream(acsfit_ctx *ctx, const PipelineParams &pp, in
 }
 
 constexpr int kOneCtaSmemKb = 116;  // more than half of the 227 KB an SM offers: a second CTA cannot be resident
-template <int D, bool BINS, bool PRUNE, int RW>
+// SEL: the node-selector form of a node pass (barrier form only: it ignores the "stream" knob)
+template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false>
 static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
-    if constexpr (RW > 0 && D <= 8 && !PRUNE) {
+    if constexpr (RW > 0 && D <= 8 && !PRUNE && !SEL) {
         if (stream_form_ok(ctx, D, RW, pp.Tn)) return launch_stream<D, BINS, RW>(ctx, pp, stages, st, resident);
     }
     constexpr int NT = stage_threads(D, BINS);
-    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW>::bytes(pp.Tn);
+    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL>::bytes(pp.Tn);
     // D >= 8: ONE stage CTA per SM.  Whether two fit is an accident of the register allocation (the bins kernel has
     // been compiled to 128 and to 237 registers by neighbouring source revisions); at c3 a second CTA on the
     // frontier's SM costs the placement chain more than the extra resident stages give back.
     if (D >= 8) smem = std::max(smem, (size_t)kOneCtaSmemKb * 1024);
     if (ctx->smem_floor_kb > 0) smem = std::max(smem, (size_t)ctx->smem_floor_kb * 1024);  // occupancy knob
-    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW>;
+    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL>;
     if (resident) {  // only asked: how many stages does the GPU hold at once?  (cached: the query costs ~10 us)
-        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE, RW, pp.Tn);
+        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0), RW, pp.Tn);
         auto it = ctx->resident_cache.find(key);
         if (it == ctx->resident_cache.end()) {
             int per_sm = 0;
@@ -1126,7 +1166,7 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     PipelineParams q = pp;
     // more stages than the GPU holds at once: several waves, each streaming the whole pod list (see the kernel's publish)
     int held = 0;
-    TRY((launch_pipeline_w<D, BINS, PRUNE, RW>(ctx, pp, stages, st, &held)));
+    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL>(ctx, pp, stages, st, &held)));
     q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
     q.prof = (ctx->prof_dev && stages <= kProfStages) ? ctx->prof_dev : nullptr;
     if (q.prof) {
@@ -1143,22 +1183,37 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
 }
 
 // the instantiation is chosen by the rank layout of the call: 0 (float64 scan), 1, 2 or 4 packed words per row
-template <int D, bool BINS, bool PRUNE>
+template <int D, bool BINS, bool PRUNE, bool SEL = false>
 static acsfit_status launch_pipeline_v(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
     switch (pp.rk.nw) {
-    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0>(ctx, pp, stages, st, resident);
-    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1>(ctx, pp, stages, st, resident);
-    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2>(ctx, pp, stages, st, resident);
-    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4>(ctx, pp, stages, st, resident);
+    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL>(ctx, pp, stages, st, resident);
+    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL>(ctx, pp, stages, st, resident);
+    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL>(ctx, pp, stages, st, resident);
+    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL>(ctx, pp, stages, st, resident);
     default: return fail(ctx, ACSFIT_E_INVALID, "rank layout with %d words", pp.rk.nw);
     }
+}
+
+// node pass with node selectors (pp.node_match != nullptr): the same pruning rule as below, barrier form only
+template <int D>
+static acsfit_status launch_pipeline_sel(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
+{
+    int prune = ctx->prune;
+    if (prune < 0) {
+        int resident = 0;
+        TRY((launch_pipeline_v<D, false, false, true>(ctx, pp, stages, st, &resident)));
+        prune = stages > resident;
+    }
+    if (prune) return launch_pipeline_v<D, false, true, true>(ctx, pp, stages, st, nullptr);
+    return launch_pipeline_v<D, false, false, true>(ctx, pp, stages, st, nullptr);
 }
 
 template <int D, bool BINS>
 static acsfit_status launch_pipeline_t(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
     if (!BINS) {
+        if (pp.node_match) return launch_pipeline_sel<D>(ctx, pp, stages, st);
         // Stage bounds + scan-list pruning (the PRUNE instantiation) pay when the pass is throughput-bound, i.e.
         // when there are more stages than the GPU holds at once (waves); a pass that fits is bound by its
         // placement chain and runs the plain instantiation.  ACSFIT_PRUNE=0/1 forces either.
@@ -1588,6 +1643,7 @@ static void reset_stats(acsfit_ctx *ctx)
     ctx->last_ms = 0.0;
     ctx->last_decisions = 0;
     ctx->last_stages = ctx->last_tiles = 0;
+    ctx->last_sel_hits = 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1600,9 +1656,11 @@ static size_t first_fit_scratch(const acsfit_ctx *ctx, int64_t P, int64_t N)
     return 8192 + sizeof(uint32_t) * (size_t)((P + 31) / 32) + sizeof(int) * (stages + 8);
 }
 
+// pod_class / node_match (device, both or neither): node selectors (the SEL form of the node pass; single GPU only)
 static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const int32_t *pod_idx, int64_t P, int D,
                                     const double *cap_type, const int32_t *node_type, double *used, int64_t N,
-                                    int32_t *out_placed, unsigned long long *out_decisions, cudaStream_t st)
+                                    int32_t *out_placed, unsigned long long *out_decisions, cudaStream_t st,
+                                    const uint8_t *pod_class = nullptr, const unsigned long long *node_match = nullptr)
 {
     if (ctx->world > 1)
         return cluster_first_fit(ctx, req, pod_idx, P, D, cap_type, node_type, used, N, out_placed, out_decisions, st);
@@ -1644,6 +1702,15 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
     pp.drained = drained;
     pp.watchdog_ns = (unsigned long long)ctx->watchdog_ms * 1000000ull;
     pp.rk = ctx->rk;
+    pp.pod_class = pod_class;
+    pp.node_match = node_match;
+    unsigned long long *hits = nullptr;
+    if (node_match) {
+        hits = arena_take<unsigned long long>(ctx, 1);
+        if (!hits) return fail(ctx, ACSFIT_E_NOMEM, "scratch arena too small for hits");
+        CUDA_TRY(cudaMemsetAsync(hits, 0, sizeof(unsigned long long), st));
+        pp.sel_hits = hits;
+    }
 
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
     TRY(launch_pipeline<false>(ctx, D, pp, plan.stages, st));
@@ -1653,6 +1720,11 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
         ++ctx->launches;
     }
     TRY(check_pipeline_status(ctx, status, st));
+    if (hits) {
+        unsigned long long h = 0;
+        CUDA_TRY(cudaMemcpy(&h, hits, sizeof h, cudaMemcpyDeviceToHost));
+        ctx->last_sel_hits += h;
+    }
     ctx->last_stages += plan.stages;
     ctx->last_tiles += pp.num_tiles;
     if (ctx->timing) {
@@ -1702,8 +1774,11 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                                   const int32_t *pool_max, const uint8_t *pool_ignored, int T, int64_t over_provision,
                                   int64_t *out_new_size, int64_t *out_units_needed, int64_t *out_bins_opened,
                                   int32_t *out_acc_pool, int32_t *out_bin_of, int64_t *out_unaccounted,
-                                  uint64_t *out_evals, cudaStream_t st, const FirstPassDone *pre = nullptr)
+                                  uint64_t *out_evals, cudaStream_t st, const FirstPassDone *pre = nullptr,
+                                  const uint8_t *pod_class = nullptr, const uint64_t *pool_match_host = nullptr)
 {
+    // pod_class [dev] (indexed like req rows) + pool_match_host [host] T (visiting order): node selectors.  They only
+    // change the pool gate: every bin of a pool carries the pool's labels, so the bin passes are the plain ones.
     for (int i = 0; i < T * D; ++i)
         if (!std::isfinite(unit_host[i])) return fail(ctx, ACSFIT_E_DOMAIN, "fulfill_pending: non-finite unit capacity");
     const int64_t alive_words = (Pp + 31) / 32;
@@ -1749,8 +1824,13 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
             evals += (uint64_t)unique_unaccounted + pre->evals;
         } else if (Pp > 0) {
             // pool gate (scaler.py:134) over the not-yet-accounted pods -> ordered list of eligible pods
-            eligible_kernel<<<grid_for(ctx, Pp, 256), 256, 0, st>>>(req, row_map, Pp, D, unit_dev + (size_t)t * D,
-                                                                   out_acc_pool, elig);
+            if (pod_class)
+                eligible_sel_kernel<<<grid_for(ctx, Pp, 256), 256, 0, st>>>(req, row_map, Pp, D, unit_dev + (size_t)t * D,
+                                                                           (unsigned long long)pool_match_host[t], pod_class,
+                                                                           out_acc_pool, elig);
+            else
+                eligible_kernel<<<grid_for(ctx, Pp, 256), 256, 0, st>>>(req, row_map, Pp, D, unit_dev + (size_t)t * D,
+                                                                       out_acc_pool, elig);
             ++ctx->launches;
             evals += (uint64_t)unique_unaccounted;
             TRY(compact(ctx, FlagPred{elig}, Pp, nullptr, list_a, block_counts, total_dev, &E, st));
@@ -2120,7 +2200,7 @@ extern "C" acsfit_status acsfit_maintain_actions(acsfit_ctx *ctx, uint8_t *io_st
 
 // resident stage CTAs the device can hold for the nodes pipeline (all of them must be running before a
 // chained bins pipeline may spin on their progress counters)
-template <int D, bool BINS>
+template <int D, bool BINS, bool SEL = false>
 static int stage_capacity_t(acsfit_ctx *ctx, int Tn)
 {
     PipelineParams q;
@@ -2128,18 +2208,24 @@ static int stage_capacity_t(acsfit_ctx *ctx, int Tn)
     q.Tn = Tn;
     q.rk = ctx->rk;
     int resident = 0;  // a chained pass fits the GPU, hence runs unpruned
-    if (launch_pipeline_v<D, BINS, false>(ctx, q, 0, nullptr, &resident) != ACSFIT_OK) return 0;
+    if (launch_pipeline_v<D, BINS, false, SEL>(ctx, q, 0, nullptr, &resident) != ACSFIT_OK) return 0;
     return resident;
 }
+template <int D>
+static int chained_capacity_t(acsfit_ctx *ctx, int Tn_nodes, int Tn_bins, bool sel)
+{
+    const int nodes = sel ? stage_capacity_t<D, false, true>(ctx, Tn_nodes) : stage_capacity_t<D, false>(ctx, Tn_nodes);
+    return std::min(nodes, stage_capacity_t<D, true>(ctx, Tn_bins));
+}
 // stage CTAs of BOTH pipelines that can be resident together (conservatively: the smaller of the two
-// per-kernel occupancies, slots taken as interchangeable)
-static int chained_capacity(acsfit_ctx *ctx, int D, int Tn_nodes, int Tn_bins)
+// per-kernel occupancies, slots taken as interchangeable); sel: the node pass is the node-selector form
+static int chained_capacity(acsfit_ctx *ctx, int D, int Tn_nodes, int Tn_bins, bool sel)
 {
     switch (D) {
-    case 2: return std::min(stage_capacity_t<2, false>(ctx, Tn_nodes), stage_capacity_t<2, true>(ctx, Tn_bins));
-    case 4: return std::min(stage_capacity_t<4, false>(ctx, Tn_nodes), stage_capacity_t<4, true>(ctx, Tn_bins));
-    case 8: return std::min(stage_capacity_t<8, false>(ctx, Tn_nodes), stage_capacity_t<8, true>(ctx, Tn_bins));
-    case 16: return std::min(stage_capacity_t<16, false>(ctx, Tn_nodes), stage_capacity_t<16, true>(ctx, Tn_bins));
+    case 2: return chained_capacity_t<2>(ctx, Tn_nodes, Tn_bins, sel);
+    case 4: return chained_capacity_t<4>(ctx, Tn_nodes, Tn_bins, sel);
+    case 8: return chained_capacity_t<8>(ctx, Tn_nodes, Tn_bins, sel);
+    case 16: return chained_capacity_t<16>(ctx, Tn_nodes, Tn_bins, sel);
     default: return 0;
     }
 }
@@ -2153,14 +2239,15 @@ static acsfit_status first_fit_chained(acsfit_ctx *ctx, const double *req, const
                                        const double *cap_type, const int32_t *node_type, double *used, int64_t N,
                                        int32_t *placed_f, unsigned long long *decisions_dev,
                                        int pool, const double *unit_row_dev, int32_t *bins_f, int64_t *bins_covered,
-                                       uint64_t *bin_evals, bool *did, cudaStream_t st)
+                                       uint64_t *bin_evals, bool *did, cudaStream_t st,
+                                       const uint8_t *pod_class = nullptr, const unsigned long long *node_match = nullptr)
 {
     *did = false;
     const StagePlan pn = plan_stages(ctx, N, 0, D, false);
     StagePlan pb = plan_stages(ctx, F, bin_pass_cap(ctx), D, true);
     // every stage CTA of both pipelines must be resident at the same time: the bins stages spin on the node
     // stages' counters, and the two grids are dispatched in no particular order
-    const int room = chained_capacity(ctx, D, pn.Tn, pb.Tn) - pn.stages - 4;  // a little headroom
+    const int room = chained_capacity(ctx, D, pn.Tn, pb.Tn, node_match != nullptr) - pn.stages - 4;  // a little headroom
     if (room < 8) return ACSFIT_OK;  // node stages (nearly) fill the device: no chaining
     pb.stages = std::min(pb.stages, room);
     const int64_t alive_words = (F + 31) / 32;
@@ -2200,6 +2287,14 @@ static acsfit_status first_fit_chained(acsfit_ctx *ctx, const double *req, const
     a.rk = ctx->rk;
 
     PipelineParams b = a;
+    a.pod_class = pod_class;  // (the node pass only: the caller checked that every pod matches the pool)
+    a.node_match = node_match;
+    unsigned long long *hits = nullptr;
+    if (node_match) {
+        TAKE(hits_dev, unsigned long long, 1);
+        CUDA_TRY(cudaMemsetAsync(hits_dev, 0, sizeof(unsigned long long), st));
+        a.sel_hits = hits = hits_dev;
+    }
     b.placed = bins_f;
     b.cap_type = nullptr;
     b.node_type = nullptr;
@@ -2233,6 +2328,11 @@ static acsfit_status first_fit_chained(acsfit_ctx *ctx, const double *req, const
     unsigned long long ev = 0;
     CUDA_TRY(cudaMemcpyAsync(&ev, evals_dev, sizeof ev, cudaMemcpyDeviceToHost, st));
     TRY(check_pipeline_status(ctx, a.status, st));
+    if (hits) {
+        unsigned long long h = 0;
+        CUDA_TRY(cudaMemcpy(&h, hits, sizeof h, cudaMemcpyDeviceToHost));
+        ctx->last_sel_hits += h;
+    }
     ctx->last_stages += pn.stages + pb.stages;
     ctx->last_tiles += 2 * a.num_tiles;
     if (ctx->timing) {
@@ -2285,9 +2385,11 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
                                    const double *cap_type, const int32_t *node_type, double *used, int64_t N,
                                    uint8_t *out_feasible, int32_t *out_placed, int64_t *out_new_size,
                                    int64_t *out_units_needed, int64_t *out_bins_opened, int32_t *out_acc_pool,
-                                   uint64_t *out_counters, cudaStream_t st)
+                                   uint64_t *out_counters, cudaStream_t st, const acsfit_selectors *sel = nullptr)
 {
     const int nblocks = (int)((P + kCompactChunk - 1) / kCompactChunk) + 1;
+    const uint8_t *pod_class = sel ? sel->pod_class : nullptr;
+    const unsigned long long *node_match = sel ? reinterpret_cast<const unsigned long long *>(sel->node_match) : nullptr;
     TAKE(flag, int, 1);
     TAKE(unit_all_dev, double, (size_t)T * D);
     TAKE(list_f, int32_t, P);      // pods to schedule (feasible), in order
@@ -2306,12 +2408,21 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
     // get_pods_to_schedule (cluster.py:217-240)
     CUDA_TRY(cudaMemsetAsync(evals_dev, 0, 2 * sizeof(unsigned long long), st));
     int64_t F = 0;
-    if (P > 0) {
+    if (P > 0 && sel) {
+        TAKE(match_all_dev, unsigned long long, T);
+        if (T > 0) CUDA_TRY(cudaMemcpyAsync(match_all_dev, sel->pool_match_all, sizeof(uint64_t) * T, cudaMemcpyHostToDevice, st));
+        feasible_mask_sel_kernel<<<grid_for(ctx, P, 256), 256, (sizeof(double) * D + sizeof(uint64_t)) * std::max(1, T), st>>>(
+            req, P, D, unit_all_dev, match_all_dev, T, pod_class, out_feasible, evals_dev);
+        ++ctx->launches;
+    } else if (P > 0) {
         feasible_mask_kernel<<<grid_for(ctx, P, 256), 256, sizeof(double) * std::max(1, T * D), st>>>(
             req, P, D, unit_all_dev, T, out_feasible, evals_dev);
+        ++ctx->launches;
+    }
+    if (P > 0) {
         expand_placed_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(out_feasible, P, out_placed);
         fill_i32_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(out_acc_pool, P, -1);
-        ctx->launches += 3;
+        ctx->launches += 2;
         TRY(compact(ctx, FlagPred{out_feasible}, P, nullptr, list_f, block_counts, total_dev, &F, st));
     }
     // get_pending_pods (cluster.py:184-204); when every pod to schedule is eligible for the first pool the
@@ -2330,8 +2441,13 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
             TAKE(inel_dev, unsigned long long, 1);
             CUDA_TRY(cudaMemcpyAsync(unit_ord_dev, unit_ordered_host, sizeof(double) * T * D, cudaMemcpyHostToDevice, st));
             CUDA_TRY(cudaMemsetAsync(inel_dev, 0, sizeof(unsigned long long), st));
-            count_ineligible_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(out_feasible, req, P, D,
-                                                                          unit_ord_dev + (size_t)t0 * D, inel_dev);
+            if (sel)
+                count_ineligible_sel_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(
+                    out_feasible, req, P, D, unit_ord_dev + (size_t)t0 * D,
+                    (unsigned long long)sel->pool_match_ordered[t0], pod_class, inel_dev);
+            else
+                count_ineligible_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(out_feasible, req, P, D,
+                                                                              unit_ord_dev + (size_t)t0 * D, inel_dev);
             ++ctx->launches;
             unsigned long long inel = 1;
             CUDA_TRY(cudaMemcpyAsync(&inel, inel_dev, sizeof inel, cudaMemcpyDeviceToHost, st));
@@ -2345,7 +2461,8 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
                 TAKE(used_backup, double, (size_t)N * D);
                 CUDA_TRY(cudaMemcpyAsync(used_backup, used, sizeof(double) * (size_t)N * D, cudaMemcpyDeviceToDevice, st));
                 acsfit_status cs = first_fit_chained(ctx, req, list_f, F, D, cap_type, node_type, used, N, placed_f, evals_dev + 1,
-                                                     t0, unit_ord_dev + (size_t)t0 * D, bins_f, &covered, &bev, &chained, st);
+                                                     t0, unit_ord_dev + (size_t)t0 * D, bins_f, &covered, &bev, &chained, st,
+                                                     pod_class, node_match);
                 if (cs == ACSFIT_OK && chained && ctx->inject_chain_timeout > 0) {  // test hook: exercise the recovery path
                     --ctx->inject_chain_timeout;
                     cs = ACSFIT_E_TIMEOUT;
@@ -2376,7 +2493,8 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
             }
         }
         if (!chained) {
-            TRY(first_fit_impl(ctx, req, list_f, F, D, cap_type, node_type, used, N, placed_f, evals_dev + 1, st));
+            TRY(first_fit_impl(ctx, req, list_f, F, D, cap_type, node_type, used, N, placed_f, evals_dev + 1, st,
+                               pod_class, node_match));
             TRY(compact(ctx, NegPred{placed_f}, F, list_f, list_p, block_counts, total_dev, &Pn, st));
         }
         scatter_i32_kernel<<<grid_for(ctx, F, 256), 256, 0, st>>>(list_f, placed_f, F, out_placed);
@@ -2397,7 +2515,7 @@ static acsfit_status scale_up_impl(acsfit_ctx *ctx, const double *req, int64_t P
         uint64_t fe = 0;
         TRY(fulfill_impl(ctx, req, list_p, Pn, Pn, D, unit_ordered_host, pool_actual, pool_max, pool_ignored, T,
                          over_provision, out_new_size, out_units_needed, out_bins_opened, acc_p, bin_p, &unaccounted,
-                         &fe, st, chained ? &pre : nullptr));
+                         &fe, st, chained ? &pre : nullptr, pod_class, sel ? sel->pool_match_ordered : nullptr));
         decisions += fe;
         scatter_i32_kernel<<<grid_for(ctx, Pn, 256), 256, 0, st>>>(list_p, acc_p, Pn, out_acc_pool);
         ++ctx->launches;
@@ -2446,6 +2564,168 @@ extern "C" acsfit_status acsfit_scale_up(acsfit_ctx *ctx, const double *req, int
     return scale_up_impl(ctx, req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T,
                          over_provision, cap_type, node_type, used_inout, N, out_feasible, out_placed, out_new_size,
                          out_units_needed, out_bins_opened, out_acc_pool, out_counters, st);
+}
+
+// ---------------------------------------------------------------------------------------------
+// node selectors (include/acsfit.h, acsfit_selectors): the *_sel entry points
+// ---------------------------------------------------------------------------------------------
+enum { kSelNodes = 1, kSelPoolsAll = 2, kSelPoolsOrdered = 4 };
+
+// host-side checks of the fields `need` names (pod_class is always needed when there are rows)
+static acsfit_status check_selectors_host(acsfit_ctx *ctx, const acsfit_selectors *sel, int64_t rows, int64_t N, int T,
+                                          int need, const char *what)
+{
+    if (!sel) return fail(ctx, ACSFIT_E_INVALID, "%s: selectors missing", what);
+    if (ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: node selectors are not supported in cluster mode", what);
+    if (sel->classes < 1 || sel->classes > ACSFIT_MAX_CLASSES)
+        return fail(ctx, ACSFIT_E_INVALID, "%s: %d selector classes, need 1..%d", what, sel->classes, ACSFIT_MAX_CLASSES);
+    if ((rows > 0 && !sel->pod_class) || ((need & kSelNodes) && N > 0 && !sel->node_match) ||
+        ((need & kSelPoolsAll) && T > 0 && !sel->pool_match_all) ||
+        ((need & kSelPoolsOrdered) && T > 0 && !sel->pool_match_ordered))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: selector field missing", what);
+    for (int t = 0; t < T; ++t)  // class 0 (no selector) matches every pool
+        if (((need & kSelPoolsAll) && !(sel->pool_match_all[t] & 1u)) ||
+            ((need & kSelPoolsOrdered) && !(sel->pool_match_ordered[t] & 1u)))
+            return fail(ctx, ACSFIT_E_INVALID, "%s: bit 0 (no selector) must be set in every pool mask", what);
+    return ACSFIT_OK;
+}
+
+// device-side checks: every class < sel->classes (the kernels shift a 64-bit mask by it) and, when node masks are
+// given, bit 0 (no selector) set in each of them
+static acsfit_status check_classes(acsfit_ctx *ctx, const uint8_t *pod_class, int64_t rows, int classes, int *flag_dev,
+                                   cudaStream_t st, const char *what, const uint64_t *node_match = nullptr,
+                                   int64_t N = 0)
+{
+    if (rows <= 0 && N <= 0) return ACSFIT_OK;
+    CUDA_TRY(cudaMemsetAsync(flag_dev, 0, sizeof(int), st));
+    if (rows > 0) {
+        class_check_kernel<<<grid_for(ctx, rows, 256), 256, 0, st>>>(pod_class, rows, classes, flag_dev);
+        ++ctx->launches;
+    }
+    if (node_match && N > 0) {
+        node_mask_check_kernel<<<grid_for(ctx, N, 256), 256, 0, st>>>(
+            reinterpret_cast<const unsigned long long *>(node_match), N, flag_dev);
+        ++ctx->launches;
+    }
+    int flag = 0;
+    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    if (flag & 1) return fail(ctx, ACSFIT_E_INVALID, "%s: a pod_class is >= classes (%d)", what, classes);
+    if (flag & 2) return fail(ctx, ACSFIT_E_INVALID, "%s: bit 0 (no selector) must be set in every node mask", what);
+    return ACSFIT_OK;
+}
+
+extern "C" acsfit_status acsfit_feasible_mask_sel(acsfit_ctx *ctx, const double *req, int64_t P, int D,
+                                                  const double *unit, int T, const acsfit_selectors *sel,
+                                                  uint8_t *out_mask, uint64_t *out_evals, acsfit_stream_t stream)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (P < 0 || T < 0 || T > ACSFIT_MAX_POOLS || (P > 0 && (!req || !out_mask)) || (T > 0 && !unit))
+        return fail(ctx, ACSFIT_E_INVALID, "feasible_mask_sel: bad arguments");
+    TRY(check_selectors_host(ctx, sel, P, 0, T, kSelPoolsAll, "feasible_mask_sel"));
+    if (out_evals) CUDA_TRY(cudaMemsetAsync(out_evals, 0, sizeof(uint64_t), st));
+    if (P == 0) return ACSFIT_OK;
+    TRY(arena_reserve(ctx, sizeof(uint64_t) * (size_t)T + 4096, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TAKE(match_dev, unsigned long long, T);
+    TRY(check_classes(ctx, sel->pod_class, P, sel->classes, flag, st, "feasible_mask_sel"));
+    if (T > 0) CUDA_TRY(cudaMemcpyAsync(match_dev, sel->pool_match_all, sizeof(uint64_t) * T, cudaMemcpyHostToDevice, st));
+    feasible_mask_sel_kernel<<<grid_for(ctx, P, 256), 256, (sizeof(double) * D + sizeof(uint64_t)) * std::max(1, T), st>>>(
+        req, P, D, unit, match_dev, T, sel->pod_class, out_mask, reinterpret_cast<unsigned long long *>(out_evals));
+    ++ctx->launches;
+    CUDA_TRY(cudaGetLastError());
+    return ACSFIT_OK;
+}
+
+extern "C" acsfit_status acsfit_first_fit_nodes_sel(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                    const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                    const int32_t *node_type, double *used_inout, int64_t N,
+                                                    const acsfit_selectors *sel, int32_t *out_placed,
+                                                    uint64_t *out_decisions, acsfit_stream_t stream)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
+        (P > 0 && (!req || !out_placed)) || (N > 0 && (!cap_type || !node_type || !used_inout)))
+        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_sel: bad arguments");
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_sel: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
+    TRY(check_req_aligned(ctx, req, "first_fit_nodes_sel"));
+    TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, "first_fit_nodes_sel"));
+    reset_stats(ctx);
+    TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_domain(ctx, req, req_rows * D, flag, st, "req"));
+    TRY(check_classes(ctx, sel->pod_class, req_rows, sel->classes, flag, st, "first_fit_nodes_sel", sel->node_match, N));
+    if (P > 0 && N > 0) TRY(build_ranks(ctx, req, req_rows, D, st));
+    return first_fit_impl(ctx, req, pod_idx, P, D, cap_type, node_type, used_inout, N, out_placed,
+                          reinterpret_cast<unsigned long long *>(out_decisions), st, sel->pod_class,
+                          reinterpret_cast<const unsigned long long *>(sel->node_match));
+}
+
+extern "C" acsfit_status acsfit_fulfill_pending_sel(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                    int64_t num_listed, int D, const double *unit,
+                                                    const int32_t *pool_actual, const int32_t *pool_max,
+                                                    const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                    const acsfit_selectors *sel, int64_t *out_new_size,
+                                                    int64_t *out_units_needed, int64_t *out_bins_opened,
+                                                    int32_t *out_acc_pool, int32_t *out_bin_of,
+                                                    int64_t *out_unaccounted, uint64_t *out_evals,
+                                                    acsfit_stream_t stream)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
+        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
+        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
+                   !out_bins_opened)) ||
+        !out_unaccounted)
+        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_sel: bad arguments");
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_sel: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
+    TRY(check_req_aligned(ctx, req, "fulfill_pending_sel"));
+    TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, "fulfill_pending_sel"));
+    reset_stats(ctx);
+    TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_domain(ctx, req, Pp * D, flag, st, "req"));
+    TRY(check_classes(ctx, sel->pod_class, Pp, sel->classes, flag, st, "fulfill_pending_sel"));
+    TRY(build_ranks(ctx, req, Pp, D, st));
+    return fulfill_impl(ctx, req, nullptr, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                        over_provision, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
+                        out_unaccounted, out_evals, st, nullptr, sel->pod_class, sel->pool_match_ordered);
+}
+
+extern "C" acsfit_status acsfit_scale_up_sel(acsfit_ctx *ctx, const double *req, int64_t P, int D,
+                                             const double *unit_all, const double *unit_ordered,
+                                             const int32_t *pool_actual, const int32_t *pool_max,
+                                             const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                             const double *cap_type, const int32_t *node_type, double *used_inout,
+                                             int64_t N, const acsfit_selectors *sel, uint8_t *out_feasible,
+                                             int32_t *out_placed, int64_t *out_new_size, int64_t *out_units_needed,
+                                             int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                             uint64_t *out_counters, acsfit_stream_t stream)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    TRY(scale_up_check(ctx, req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T, cap_type,
+                       node_type, used_inout, N, out_feasible, out_placed, out_new_size, out_units_needed,
+                       out_bins_opened, out_acc_pool, out_counters));
+    TRY(check_req_aligned(ctx, req, "scale_up_sel"));
+    TRY(check_selectors_host(ctx, sel, P, N, T, kSelNodes | kSelPoolsAll | kSelPoolsOrdered, "scale_up_sel"));
+    reset_stats(ctx);
+    TRY(arena_reserve(ctx, scale_up_scratch(ctx, P, N, T, D) + sizeof(uint64_t) * (size_t)T + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_classes(ctx, sel->pod_class, P, sel->classes, flag, st, "scale_up_sel", sel->node_match, N));
+    return scale_up_impl(ctx, req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T,
+                         over_provision, cap_type, node_type, used_inout, N, out_feasible, out_placed, out_new_size,
+                         out_units_needed, out_bins_opened, out_acc_pool, out_counters, st, sel);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2526,6 +2806,65 @@ extern "C" acsfit_status acsfit_scale_up_host(acsfit_ctx *ctx, const double *req
     TRY(scale_up_impl(ctx, d_req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T, over_provision,
                       d_cap, d_type, d_used, N, d_feas, d_placed, out_new_size, out_units_needed, out_bins_opened,
                       d_acc, out_counters, st));
+    D2H(out_feasible, d_feas, (size_t)P);
+    D2H(out_placed, d_placed, sizeof(int32_t) * (size_t)P);
+    D2H(out_acc_pool, d_acc, sizeof(int32_t) * (size_t)P);
+    D2H(used_inout, d_used, sizeof(double) * (size_t)N * D);
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return ACSFIT_OK;
+}
+
+// the same with node selectors; sel->pod_class and sel->node_match are host pointers here
+extern "C" acsfit_status acsfit_scale_up_sel_host(acsfit_ctx *ctx, const double *req, int64_t P, int D,
+                                                  const double *unit_all, const double *unit_ordered,
+                                                  const int32_t *pool_actual, const int32_t *pool_max,
+                                                  const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                  const double *cap_type, int K, const int32_t *node_type,
+                                                  double *used_inout, int64_t N, const acsfit_selectors *sel,
+                                                  uint8_t *out_feasible, int32_t *out_placed,
+                                                  int64_t *out_new_size, int64_t *out_units_needed,
+                                                  int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                                  uint64_t *out_counters)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = nullptr;
+    if (K < 0) return fail(ctx, ACSFIT_E_INVALID, "scale_up_sel_host: K < 0");
+    TRY(scale_up_check(ctx, req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T, cap_type,
+                       node_type, used_inout, N, out_feasible, out_placed, out_new_size, out_units_needed,
+                       out_bins_opened, out_acc_pool, out_counters));
+    TRY(check_selectors_host(ctx, sel, P, N, T, kSelNodes | kSelPoolsAll | kSelPoolsOrdered, "scale_up_sel_host"));
+    for (int i = 0; i < K * D; ++i)
+        if (!std::isfinite(cap_type[i])) return fail(ctx, ACSFIT_E_DOMAIN, "scale_up_sel_host: non-finite capacity");
+    reset_stats(ctx);
+    const size_t bytes = sizeof(double) * ((size_t)P * D + (size_t)K * D + (size_t)N * D) +
+                         sizeof(int32_t) * ((size_t)N + 2 * (size_t)P) + 2 * (size_t)P + sizeof(uint64_t) * (size_t)N +
+                         16 * 256;
+    TRY(hbuf_reserve(ctx, bytes));
+    HTAKE(d_req, double, (size_t)P * D);
+    HTAKE(d_cap, double, (size_t)K * D);
+    HTAKE(d_used, double, (size_t)N * D);
+    HTAKE(d_type, int32_t, N);
+    HTAKE(d_placed, int32_t, P);
+    HTAKE(d_acc, int32_t, P);
+    HTAKE(d_feas, uint8_t, P);
+    HTAKE(d_class, uint8_t, P);
+    HTAKE(d_match, uint64_t, N);
+    H2D(d_req, req, sizeof(double) * (size_t)P * D);
+    H2D(d_cap, cap_type, sizeof(double) * (size_t)K * D);
+    H2D(d_used, used_inout, sizeof(double) * (size_t)N * D);
+    H2D(d_type, node_type, sizeof(int32_t) * (size_t)N);
+    H2D(d_class, sel->pod_class, (size_t)P);
+    H2D(d_match, sel->node_match, sizeof(uint64_t) * (size_t)N);
+    acsfit_selectors dsel = *sel;
+    dsel.pod_class = d_class;
+    dsel.node_match = d_match;
+    TRY(arena_reserve(ctx, scale_up_scratch(ctx, P, N, T, D) + sizeof(uint64_t) * (size_t)T + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_classes(ctx, d_class, P, sel->classes, flag, st, "scale_up_sel_host", d_match, N));
+    TRY(scale_up_impl(ctx, d_req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T, over_provision,
+                      d_cap, d_type, d_used, N, d_feas, d_placed, out_new_size, out_units_needed, out_bins_opened,
+                      d_acc, out_counters, st, &dsel));
     D2H(out_feasible, d_feas, (size_t)P);
     D2H(out_placed, d_placed, sizeof(int32_t) * (size_t)P);
     D2H(out_acc_pool, d_acc, sizeof(int32_t) * (size_t)P);

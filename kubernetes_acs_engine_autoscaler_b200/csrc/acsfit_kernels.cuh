@@ -126,6 +126,12 @@ struct PipelineParams {
     unsigned long long *prof;  // optional [stages][8] clock64 phase totals (developer probe), or nullptr
     unsigned long long *trace; // optional [num_tiles][8] per-tile trace of stage `trace_stage`
     int trace_stage;
+    // node selectors (SEL instantiations of a node pass only; appended so that no other field moves):
+    // a pod may take a node only when bit pod_class[row] of node_match[node] is set (class 0 = no selector,
+    // its bit is set in every mask)
+    const uint8_t *pod_class;               // [req rows] selector class of each request row
+    const unsigned long long *node_match;   // [N] classes each node matches
+    unsigned long long *sel_hits;           // optional: += the scan's hit entries of every tile of every stage
 };
 
 __device__ __forceinline__ int ld_acquire(const int *p)
@@ -194,7 +200,7 @@ __device__ __forceinline__ void load_row(double (&r)[D], const double *src)
 // dynamic shared memory layout (doubles first for alignment).
 // nodes mode keeps three [D][Tn] arrays: scan thresholds, used (the mutable state) and capacity;
 // bins mode keeps one: the remaining capacity IS the threshold (finite values, Lemma B).
-template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0>
+template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false>
 struct PipelineSmem {
     static constexpr int NW = NT / 32;  // warps per stage CTA == resolver warps
     static __host__ __device__ size_t bytes(int Tn)
@@ -204,7 +210,8 @@ struct PipelineSmem {
                                      NW /*dirty*/ + 8 /*scan counts*/ + 8 /*alive counts*/ + 8 /*misc*/ + kRing * 8 /*alive words of the next tiles*/ + (kTile + 1) /*hitlist*/ +
                                      (NW - 1) * (kTile + 1) /*warp queues*/ + 1 /*pad*/)
                + sizeof(unsigned short) * kTile /*slot_of*/ + (size_t)NW * 32 /*accepted node per dense entry*/
-               + sizeof(unsigned) * ((size_t)RW * Tn /*packed node words*/ + (size_t)RW * kTile /*packed pod words*/ + 4 /*alignment*/);
+               + sizeof(unsigned) * ((size_t)RW * Tn /*packed node words*/ + (size_t)RW * kTile /*packed pod words*/ + 4 /*alignment*/)
+               + (SEL ? sizeof(unsigned long long) * (size_t)Tn /*node masks*/ + kTile /*pod classes*/ + (size_t)NW * 36 /*batch classes*/ : 0);
     }
 };
 
@@ -236,10 +243,18 @@ __device__ __forceinline__ unsigned wait_entry(const volatile unsigned *slot, in
 
 // D <= 4: two stage CTAs per SM are part of the design (the node and the bin launch of a tick run chained, both resident),
 // so the register budget is pinned to 128 instead of being left to the allocator's mood; D >= 8 runs one CTA per SM.
-template <int D, bool BINS, int NT, bool PRUNE, int RW>
+//
+// SEL (node passes only): node selectors.  A pod may take a node only when bit pod_class of the node's match mask is
+// set.  The predicate is static per (pod, node) pair, so it is ANDed into both candidate scans and into the resolver's
+// vote, and everything else keeps its meaning: a node's threshold only shrinks, so a stale threshold is still a
+// superset filter of "fits AND matches"; the per-warp and per-stage bounds stay resource-only (see the PRUNE test in
+// the tile loader).  Bin passes need no SEL form: every bin of a pool carries the pool's labels, so the host gates the
+// pods by match before a bin pass and the "untouched bin takes every eligible pod" shortcut stays exact.
+template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false>
 __global__ void __launch_bounds__(NT, D <= 4 ? 2 : 1)
 firstfit_pipeline_kernel(const PipelineParams p)
 {
+    static_assert(!(SEL && BINS), "selectors apply to node passes only");
     constexpr int K = nodes_per_thread(D, RW);  // RW: 32-bit words of a packed-rank row, 0 = float64 scan
     constexpr int NW = NT / 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -267,6 +282,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
     // packed-rank rows (RW > 0): scan thresholds of the stage's nodes and the compacted pods of the tile
     unsigned *tw_s = reinterpret_cast<unsigned *>((reinterpret_cast<uintptr_t>(found_s + NW * 32) + 15) & ~(uintptr_t)15);  // [Tn][RW]
     unsigned *rw_s = tw_s + (size_t)RW * Tn;                                                                              // [kTile][RW]
+    // SEL: match masks of the stage's nodes, classes of the tile's compacted pods and of each resolver batch
+    // (rw_s + RW * kTile is 16-byte aligned: tw_s is, and RW * (Tn + kTile) words are a multiple of 4)
+    unsigned long long *nm_s = reinterpret_cast<unsigned long long *>(rw_s + (size_t)RW * kTile);  // [Tn]
+    unsigned char *cls_s = reinterpret_cast<unsigned char *>(nm_s + Tn);                           // [kTile]
+    unsigned char *bcls_s = cls_s + kTile;                                                         // [NW][36]
 
     const int tid = threadIdx.x;
     const int lane = tid & 31;
@@ -321,6 +341,8 @@ firstfit_pipeline_kernel(const PipelineParams p)
     for (int i = tid; i < NW * (kTile + 1) + 1; i += NT) hitlist[i] = 0;  // hit list + the NW-1 queues
     if constexpr (RW > 0)
         for (int i = tid; i < Tn * RW; i += NT) tw_s[i] = 0;
+    if constexpr (SEL)  // padding nodes match nothing (they never fit either)
+        for (int n = tid; n < Tn; n += NT) nm_s[n] = n < n_valid ? __ldg(p.node_match + stage_lo + n) : 0ull;
     __syncthreads();
     // (n, d) -> field t' of the node's packed threshold row; callers zero the row first
     auto pack_field = [&](int i) {
@@ -386,6 +408,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
     // while the current tile is scanned; only the alive word has to wait for the upstream stage.
     double pre[D];
     unsigned prew[RW > 0 ? RW : 1];
+    unsigned pre_cls = 0;  // SEL: the entry's selector class
     auto prefetch_row = [&](int tile) {
         const int64_t j = (int64_t)(p.tile_lo + tile) * kTile + tid;
         if (tid < kTile && tile < p.num_tiles && j < p.M) {
@@ -402,6 +425,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
 #pragma unroll
                 for (int w = 0; w < RW; ++w) prew[w] = __ldg(p.rk.packed + (size_t)row * RW + w);
             }
+            if constexpr (SEL) pre_cls = __ldg(p.pod_class + row);
         }
     };
     prefetch_row(0);
@@ -464,6 +488,9 @@ firstfit_pipeline_kernel(const PipelineParams p)
         const unsigned word = nextw[(tile % kRing) * (kTile / 32) + warp];
         const bool is_alive = (word >> lane) & 1u;
         bool pass = is_alive;
+        // SEL: the bounds stay resource-only.  A pod they prune exceeds, in some dimension, every threshold of the
+        // stage, so it fits no node here whatever the node matches: leaving it out is exact.  A pod that passes
+        // only because a node it does not match has room is scanned in vain, which costs time, never a result.
         if (PRUNE && is_alive) {  // can the pod fit any node of the stage at all?  (per-dimension bound over the warps)
 #pragma unroll
             for (int d = 0; d < D; ++d) pass = pass & (pre[d] <= smax[d]);
@@ -513,6 +540,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
 #pragma unroll
                 for (int w = 0; w < RW; ++w) rw_s[pos * RW + w] = prew[w];
             }
+            if constexpr (SEL) cls_s[pos] = (unsigned char)pre_cls;
         }
         prefetch_row(tile + 1);
         __syncthreads();
@@ -539,9 +567,14 @@ firstfit_pipeline_kernel(const PipelineParams p)
             for (int k = 0; k < K; ++k)
 #pragma unroll
                 for (int w = 0; w < RW; ++w) tg[k][w] = tw_s[(slot + k * NS) * RW + w] | g[w];
+            unsigned long long nm[SEL ? K : 1];  // SEL: match masks of this thread's nodes
+            if constexpr (SEL) {
+#pragma unroll
+                for (int k = 0; k < K; ++k) nm[k] = nm_s[slot + k * NS];
+            }
             constexpr int PPI = 4;  // pods per thread and iteration
             for (unsigned qb = 0; qb < total; qb += PPI * PG) {
-                unsigned q[PPI], best[PPI], r[PPI][RW];
+                unsigned q[PPI], best[PPI], r[PPI][RW], c[PPI];
                 bool live[PPI];
 #pragma unroll
                 for (int i = 0; i < PPI; ++i) {
@@ -550,6 +583,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     const unsigned *src = rw_s + (size_t)(live[i] ? q[i] : total - 1) * RW;
 #pragma unroll
                     for (int w = 0; w < RW; ++w) r[i][w] = src[w];
+                    if constexpr (SEL) c[i] = cls_s[live[i] ? q[i] : total - 1];
                     best[i] = kNoCand;
                 }
 #pragma unroll
@@ -559,7 +593,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         unsigned miss = 0;
 #pragma unroll
                         for (int w = 0; w < RW; ++w) miss |= ((tg[k][w] - r[i][w]) & g[w]) ^ g[w];
-                        if (miss == 0 && live[i]) best[i] = (unsigned)(slot + k * NS);
+                        if constexpr (SEL) {
+                            if (miss == 0 && live[i] && ((nm[k] >> c[i]) & 1ull)) best[i] = (unsigned)(slot + k * NS);
+                        } else {
+                            if (miss == 0 && live[i]) best[i] = (unsigned)(slot + k * NS);
+                        }
                     }
                 }
                 unsigned any_best = best[0];
@@ -588,12 +626,17 @@ firstfit_pipeline_kernel(const PipelineParams p)
             for (int k = 0; k < K; ++k)
 #pragma unroll
                 for (int d = 0; d < D; ++d) t[k][d] = thr_s[(size_t)d * Tn + slot + k * NS];
+            unsigned long long nm[SEL ? K : 1];  // SEL: match masks of this thread's nodes
+            if constexpr (SEL) {
+#pragma unroll
+                for (int k = 0; k < K; ++k) nm[k] = nm_s[slot + k * NS];
+            }
             // several pods per iteration: their compares are independent, which keeps the fp64 pipe fed with
             // only eight warps per stage, and the vote / loop overhead is paid once per group of pods;
             // trip count is warp-uniform (votes inside)
             constexpr int PPI = (D == 8) ? 4 : 2;  // pods per thread and iteration
             for (unsigned qb = 0; qb < total; qb += PPI * PG) {
-                unsigned q[PPI];
+                unsigned q[PPI], c[PPI];
                 bool live[PPI];
                 double r[PPI][D];
                 unsigned best[PPI];
@@ -602,6 +645,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     q[i] = qb + (unsigned)(i * PG + group);
                     live[i] = q[i] < total;
                     load_row<D>(r[i], rows + (size_t)(live[i] ? q[i] : total - 1) * D);
+                    if constexpr (SEL) c[i] = cls_s[live[i] ? q[i] : total - 1];
                     best[i] = kNoCand;
                 }
 #pragma unroll
@@ -611,6 +655,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         bool ok = live[i];
 #pragma unroll
                         for (int d = 0; d < D; ++d) ok = ok & (r[i][d] <= t[k][d]);
+                        if constexpr (SEL) ok = ok & (((nm[k] >> c[i]) & 1ull) != 0ull);
                         if (ok) best[i] = (unsigned)(slot + k * NS);
                     }
                 }
@@ -676,6 +721,12 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 if (tid == 0) hitlist[ht] = kQueueEnd;
             }
         }
+        // SEL: count the pods the scan handed to the resolver (pods with a candidate node that fits AND matches);
+        // the count is exposed so that a scan whose match filter stopped working is caught by a test, although the
+        // resolver's own match test keeps every placement right
+        if constexpr (SEL) {
+            if (tid == 0 && nh && p.sel_hits) atomicAdd(p.sel_hits, (unsigned long long)nh);
+        }
         if (nh > 0) {
             __syncthreads();
             unsigned out = 0;
@@ -701,6 +752,8 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 // bins: bit per lane = the bin already holds a pod (persists over tiles); nodes: threshold is stale
                 unsigned touched_or_open = BINS ? opened[warp] : 0u;
                 unsigned touched_tile = 0u;  // nodes / bins of this warp that took a pod in this tile
+                unsigned long long my_nm = 0ull;  // SEL: the classes this lane's node matches
+                if constexpr (SEL) my_nm = n < Tn ? nm_s[n] : 0ull;
 
                 unsigned my_takes = 0;  // pods this lane's node / bin took in this tile
                 const volatile unsigned *in_q = warp == first_w ? hitlist : queue + (size_t)(warp - 1) * (kTile + 1);
@@ -777,10 +830,12 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         continue;
                     }
                     const int my_rank = __popc(possmask & ((1u << lane) - 1u));
+                    unsigned char *bcls = bcls_s + warp * 36;  // SEL: class of each dense entry (+4 padding entries)
                     if (poss) {
 #pragma unroll
                         for (int d = 0; d < D; d += 2)
                             *reinterpret_cast<double2 *>(brow + (size_t)my_rank * D + d) = make_double2(own[d], own[d + 1]);
+                        if constexpr (SEL) bcls[my_rank] = cls_s[q_l];
                     }
                     fnd[lane] = 0xFF;  // "nobody took dense entry `lane`" until a taker says otherwise
                     const unsigned fnd_sa = (unsigned)__cvta_generic_to_shared(const_cast<unsigned char *>(fnd));
@@ -789,10 +844,15 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         pad[0] = __longlong_as_double(0x7FF0000000000000ll);
 #pragma unroll
                         for (int d = 1; d < D; ++d) pad[d] = 0.0;
+                        if constexpr (SEL) bcls[n_poss + lane] = 0;
                     }
                     __syncwarp();
                     double r[D];
                     load_row<D>(r, brow);
+                    // SEL: does this lane's node match entry k?  It does not depend on S, so it is computed one entry
+                    // ahead, beside the row load, and is ready before the add-compare-vote chain needs it.
+                    bool mt = true;
+                    if constexpr (SEL) mt = ((my_nm >> bcls[0]) & 1ull) != 0ull;
                     const long long t_l0 = tracing ? clock64() : 0;
                     if (tracing) n_iter += (unsigned)n_poss;
                     // The placement chain.  Entry k's test needs the state left by entry k-1, which is only known once the
@@ -822,7 +882,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     for (int k = k0; k < k0 + 4; ++k) {  // slots past n_poss hold never-fitting rows
                         double r_next[D];
                         load_row<D>(r_next, brow + (size_t)(k + 1) * D);
-                        const bool ok = fits(S, r);
+                        bool mt_next = true;
+                        if constexpr (SEL) mt_next = ((my_nm >> bcls[k + 1]) & 1ull) != 0ull;
+                        bool ok = fits(S, r);
+                        if constexpr (SEL) ok = ok & mt;
                         // the vote-to-vote path: ballot -> "no fitting lane before me" -> predicated update of S -> next
                         // test.  No branch on it (at the frontier nearly every entry is taken) and no mask arithmetic
                         // beyond one and + compare.
@@ -834,6 +897,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         my_takes += loses ? 0u : 1u;
 #pragma unroll
                         for (int d = 0; d < D; ++d) r[d] = r_next[d];
+                        if constexpr (SEL) mt = mt_next;
                     }
                     __syncwarp();
                     {
@@ -1022,6 +1086,58 @@ __global__ void eligible_kernel(const double *__restrict__ req, const int32_t *_
         if (acc_pool[pidx] < 0) {
             const double *r = req + (size_t)(row_map ? row_map[pidx] : pidx) * D;
             bool all = true;
+            for (int d = 0; d < D; ++d) all = all && fits_bin(unit[d], r[d]);
+            f = all ? 1 : 0;
+        }
+        out_flag[pidx] = f;
+    }
+}
+
+// K0 with node selectors: a pool counts only when it matches the pod's selector class as well; one evaluation per
+// pool visited (the match test is evaluated first and short-circuits, it is not a second evaluation)
+__global__ void feasible_mask_sel_kernel(const double *__restrict__ req, int64_t P, int D,
+                                         const double *__restrict__ unit, const unsigned long long *__restrict__ pool_match,
+                                         int T, const uint8_t *__restrict__ pod_class,
+                                         uint8_t *__restrict__ out_mask, unsigned long long *out_evals)
+{
+    extern __shared__ double unit_s[];
+    unsigned long long *match_s = reinterpret_cast<unsigned long long *>(unit_s + T * D);
+    for (int i = threadIdx.x; i < T * D; i += blockDim.x) unit_s[i] = unit[i];
+    for (int i = threadIdx.x; i < T; i += blockDim.x) match_s[i] = pool_match[i];
+    __syncthreads();
+    unsigned long long evals = 0;
+    for (int64_t pidx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; pidx < P;
+         pidx += (int64_t)gridDim.x * blockDim.x) {
+        const double *r = req + (size_t)pidx * D;
+        const unsigned c = pod_class[pidx];
+        uint8_t ok = 0;
+        for (int t = 0; t < T && !ok; ++t) {
+            ++evals;
+            bool all = ((match_s[t] >> c) & 1ull) != 0ull;
+            for (int d = 0; d < D; ++d) all = all && fits_bin(unit_s[t * D + d], r[d]);
+            ok = all ? 1 : 0;
+        }
+        out_mask[pidx] = ok;
+    }
+    if (out_evals) {
+        for (int o = 16; o > 0; o >>= 1) evals += __shfl_down_sync(0xFFFFFFFFu, evals, o);
+        if ((threadIdx.x & 31) == 0 && evals) atomicAdd(out_evals, evals);
+    }
+}
+
+// pool gate of fulfill_pending with node selectors: the pool matches the pod's class and (unit - req).possible
+__global__ void eligible_sel_kernel(const double *__restrict__ req, const int32_t *__restrict__ row_map,
+                                    int64_t P, int D, const double *__restrict__ unit /*D, device*/,
+                                    unsigned long long pool_match, const uint8_t *__restrict__ pod_class,
+                                    const int32_t *__restrict__ acc_pool, uint8_t *__restrict__ out_flag)
+{
+    for (int64_t pidx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; pidx < P;
+         pidx += (int64_t)gridDim.x * blockDim.x) {
+        uint8_t f = 0;
+        if (acc_pool[pidx] < 0) {
+            const int64_t row = row_map ? row_map[pidx] : pidx;
+            const double *r = req + (size_t)row * D;
+            bool all = ((pool_match >> pod_class[row]) & 1ull) != 0ull;
             for (int d = 0; d < D; ++d) all = all && fits_bin(unit[d], r[d]);
             f = all ? 1 : 0;
         }

@@ -156,6 +156,13 @@ class Engine(object):
         self._check(self._lib.acsfit_last_scan_launch(self._ctx, _ptr(out)))
         return dict(zip(_native.SCAN_FIELDS, (int(v) for v in out)))
 
+    def last_sel_hits(self):
+        """test hook: pods the candidate scan of the last call's selector node passes handed to the resolver (summed over
+        tiles and stages; a pod counts in a stage only when some node there fits it AND matches its selector class)."""
+        out = ctypes.c_uint64(0)
+        self._check(self._lib.acsfit_last_sel_hits(self._ctx, ctypes.cast(ctypes.byref(out), ctypes.c_void_p)))
+        return int(out.value)
+
     def debug_profile(self, enabled=True):
         """developer probe: per-stage clock64 totals [stages, 8] of the last pipeline launch
         (wait, load, scan, resolve, publish, refresh, hits, tiles)."""
@@ -279,6 +286,137 @@ class Engine(object):
                 "units_needed": units_needed, "bins_opened": bins_opened,
                 "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
                 "num_unaccounted": int(counters[2]), "decisions": int(counters[3])}
+
+    # ------------------------------------------------------------------ node selectors (include/acsfit.h)
+    @staticmethod
+    def _selectors(classes, pod_class=None, node_match=None, pool_match_all=None, pool_match_ordered=None):
+        """(struct acsfit_selectors, the arrays it points to -- keep them alive over the call).  Pool masks are host
+        arrays; pod_class / node_match are whatever the entry point expects (device tensors, or host arrays for
+        scale_up_sel_host)."""
+        keep = [None if a is None else (a if isinstance(a, torch.Tensor) else _np(a, a.dtype))
+                for a in (pod_class, node_match)]
+        keep += [None if a is None else _np(a, np.uint64) for a in (pool_match_all, pool_match_ordered)]
+        sel = _native.Selectors(*[None if a is None else _ptr(a).value for a in keep], int(classes))
+        return sel, keep
+
+    def feasible_mask_sel(self, req, unit, pod_class, pool_match, classes):
+        """feasible_mask with node selectors: pod_class uint8 [P] device, pool_match uint64 [T] host
+        (agent_pools order)."""
+        P, D = req.shape
+        T = unit.shape[0]
+        mask = self.empty((P,), torch.uint8)
+        evals = torch.zeros(1, dtype=torch.int64, device=self.device)
+        sel, keep = self._selectors(classes, pod_class=pod_class, pool_match_all=pool_match)
+        self._check(self._lib.acsfit_feasible_mask_sel(self._ctx, _ptr(req), P, D, _ptr(unit), T,
+                                                       ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(mask),
+                                                       _ptr(evals), self._stream()))
+        return mask, evals
+
+    def first_fit_nodes_sel(self, req, pod_idx, cap_type, node_type, used, pod_class, node_match, classes):
+        """first_fit_nodes with node selectors: pod_class uint8 [req rows] device, node_match uint64 [N] device."""
+        rows, D = req.shape
+        P = rows if pod_idx is None else pod_idx.shape[0]
+        N = used.shape[0]
+        placed = self.empty((P,), torch.int32)
+        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
+        sel, keep = self._selectors(classes, pod_class=pod_class, node_match=node_match)
+        self._check(self._lib.acsfit_first_fit_nodes_sel(
+            self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
+            ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(placed), _ptr(decisions), self._stream()))
+        return placed, decisions
+
+    def fulfill_pending_sel(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision,
+                            pod_class, pool_match, classes):
+        """fulfill_pending with node selectors: pod_class uint8 [Pp] device, pool_match uint64 [T] host (visiting
+        order, like every other pool array here)."""
+        Pp, D = req.shape
+        unit = _np(unit, np.float64).reshape(-1, D)
+        T = unit.shape[0]
+        pool_actual = _np(pool_actual, np.int32)
+        pool_max = _np(pool_max, np.int32)
+        pool_ignored = _np(pool_ignored, np.uint8)
+        new_size = np.zeros(T, dtype=np.int64)
+        units_needed = np.zeros(T, dtype=np.int64)
+        bins_opened = np.zeros(T, dtype=np.int64)
+        acc_pool = self.empty((Pp,), torch.int32)
+        bin_of = self.empty((Pp,), torch.int32)
+        unacc = ctypes.c_int64(0)
+        evals = ctypes.c_uint64(0)
+        sel, keep = self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
+        self._check(self._lib.acsfit_fulfill_pending_sel(
+            self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
+            _ptr(pool_ignored), T, int(over_provision), ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
+            _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(bin_of),
+            ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p), ctypes.cast(ctypes.byref(evals), ctypes.c_void_p),
+            self._stream()))
+        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
+                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
+                "evals": int(evals.value)}
+
+    def scale_up_sel(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,
+                     cap_type, node_type, used, pod_class, node_match, pool_match_all, pool_match_ordered, classes):
+        """scale_up with node selectors: pod_class uint8 [P] / node_match uint64 [N] device, the pool masks host."""
+        P, D = req.shape
+        N = used.shape[0]
+        unit_all = _np(unit_all, np.float64).reshape(-1, D)
+        unit_ordered = _np(unit_ordered, np.float64).reshape(-1, D)
+        T = unit_all.shape[0]
+        pool_actual = _np(pool_actual, np.int32)
+        pool_max = _np(pool_max, np.int32)
+        pool_ignored = _np(pool_ignored, np.uint8)
+        feasible = self.empty((P,), torch.uint8)
+        placed = self.empty((P,), torch.int32)
+        acc_pool = self.empty((P,), torch.int32)
+        new_size = np.zeros(T, dtype=np.int64)
+        units_needed = np.zeros(T, dtype=np.int64)
+        bins_opened = np.zeros(T, dtype=np.int64)
+        counters = np.zeros(4, dtype=np.uint64)
+        sel, keep = self._selectors(classes, pod_class, node_match, pool_match_all, pool_match_ordered)
+        self._check(self._lib.acsfit_scale_up_sel(
+            self._ctx, _ptr(req), P, D, _ptr(unit_all), _ptr(unit_ordered), _ptr(pool_actual), _ptr(pool_max),
+            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), _ptr(node_type), _ptr(used), N,
+            ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(feasible), _ptr(placed), _ptr(new_size),
+            _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(counters), self._stream()))
+        return {"feasible": feasible, "placed": placed, "acc_pool": acc_pool, "new_size": new_size,
+                "units_needed": units_needed, "bins_opened": bins_opened,
+                "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
+                "num_unaccounted": int(counters[2]), "decisions": int(counters[3])}
+
+    def scale_up_sel_host(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,
+                          cap_type, node_type, used, pod_class, node_match, pool_match_all, pool_match_ordered,
+                          classes):
+        """scale_up_host with node selectors: every buffer, pod_class and node_match included, is a HOST array."""
+        req = _np(req, np.float64)
+        P, D = req.shape
+        cap_type = _np(cap_type, np.float64).reshape(-1, D)
+        K = cap_type.shape[0]
+        node_type = _np(node_type, np.int32)
+        assert isinstance(used, np.ndarray) and used.dtype == np.float64 and used.flags.c_contiguous
+        N = used.shape[0]
+        unit_all = _np(unit_all, np.float64).reshape(-1, D)
+        unit_ordered = _np(unit_ordered, np.float64).reshape(-1, D)
+        T = unit_all.shape[0]
+        pool_actual = _np(pool_actual, np.int32)
+        pool_max = _np(pool_max, np.int32)
+        pool_ignored = _np(pool_ignored, np.uint8)
+        out = {"feasible": np.empty(P, dtype=np.uint8), "placed": np.empty(P, dtype=np.int32),
+               "acc_pool": np.empty(P, dtype=np.int32)}
+        new_size = np.zeros(T, dtype=np.int64)
+        units_needed = np.zeros(T, dtype=np.int64)
+        bins_opened = np.zeros(T, dtype=np.int64)
+        counters = np.zeros(4, dtype=np.uint64)
+        sel, keep = self._selectors(classes, _np(pod_class, np.uint8), _np(node_match, np.uint64), pool_match_all,
+                                    pool_match_ordered)
+        self._check(self._lib.acsfit_scale_up_sel_host(
+            self._ctx, _ptr(req), P, D, _ptr(unit_all), _ptr(unit_ordered), _ptr(pool_actual), _ptr(pool_max),
+            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), K, _ptr(node_type), _ptr(used), N,
+            ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(out["feasible"]), _ptr(out["placed"]),
+            _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(out["acc_pool"]), _ptr(counters)))
+        res = dict(out)
+        res.update({"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
+                    "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
+                    "num_unaccounted": int(counters[2]), "decisions": int(counters[3])})
+        return res
 
     # ------------------------------------------------------------------ host-buffer entry points
     def scale_up_host(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,

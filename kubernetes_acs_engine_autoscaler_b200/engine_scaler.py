@@ -21,9 +21,10 @@ ACT_NONE, ACT_CORDON_DRAIN, ACT_CORDON, ACT_UNCORDON, ACT_SCALE_IN = range(5)
 
 class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
-                 deployments, arm_template, arm_parameters, ignore_pools, notifier):
+                 deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
+        self.node_selectors = node_selectors
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)

@@ -61,6 +61,7 @@ class Scaler(object):
         self.agent_pools = None
         self.scalable_pools = None
         self.ignored_pool_names = {}
+        self.node_selectors = False  # honour the pods' nodeSelectors (Cluster(node_selectors=...))
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -81,7 +82,9 @@ class Scaler(object):
         # occurrence, but num_unaccounted starts at len(pods) (scaler.py:119-120)
         unique = list(dict((p, False) for p in pods).keys())
         ordered_pools = capacity.order_by_cost_asc(self.agent_pools)
-        res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision)
+        classes = snapshot.selector_classes(unique, [], ordered_pools) if self.node_selectors else None
+        res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision,
+                               classes=classes)
 
         new_pool_sizes, current_pool_sizes = {}, {}
         unaccounted = len(pods)
@@ -113,7 +116,14 @@ class Scaler(object):
                 raise NameError("name 'selectors_hash' is not defined")
             if self.notifier:
                 left = [p for p, t in zip(unique, acc.tolist()) if t < 0]
-                self.notifier.notify_failed_to_scale({}, left)
+                if not self.node_selectors:
+                    self.notifier.notify_failed_to_scale({}, left)
+                else:  # once per selector of the unaccounted pods, as the upstream code grouped them
+                    groups = {}
+                    for p in left:
+                        groups.setdefault(tuple(sorted(p.selectors.items())), []).append(p)
+                    for items, group in groups.items():
+                        self.notifier.notify_failed_to_scale(dict(items), group)
         self.scale_pools(new_pool_sizes)
         if self.notifier:
             self.notifier.notify_scale(new_pool_sizes, pods, current_pool_sizes)

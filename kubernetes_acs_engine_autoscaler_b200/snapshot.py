@@ -133,10 +133,77 @@ def _write_back_used(nodes, dims, used, touched_keys):
 
 
 # ------------------------------------------------------------------------------------------------
+# node selectors: match classes (include/acsfit.h, acsfit_selectors)
+# ------------------------------------------------------------------------------------------------
+MAX_SELECTOR_CLASSES = 64
+
+
+class SelectorClasses(object):
+    """pod_class uint8[P], node_match uint64[N], pool_match uint64[T] (in the order the pools were given) and the
+    number of classes.  Bit c of a mask is set when the node / pool matches the selectors of class c."""
+
+    def __init__(self, pod_class, node_match, pool_match, classes):
+        self.pod_class = pod_class
+        self.node_match = node_match
+        self.pool_match = pool_match
+        self.classes = classes
+
+    @property
+    def trivial(self):
+        """every pod is class 0 (no selector, or one that matches every node and pool)"""
+        return not self.pod_class.any()
+
+
+def _selector_matches(labels, items):
+    return all(labels.get(key) == value for key, value in items)  # KubeNode.is_match
+
+
+def selector_classes(pods, nodes, pools):
+    """map every distinct match signature (set of matching nodes, set of matching pools) of the pods' nodeSelectors
+    to a class number.  Class 0 is "no selector": it matches everything, so a selector that matches every node and
+    every pool shares it.  Pods whose selectors match the same nodes and pools share a class.  A pool matches with
+    the labels a new node of it would carry (AgentPool.labels).  Raises ValueError above 64 classes."""
+    pods, nodes, pools = list(pods), list(nodes), list(pools)
+    node_labels = [n.selectors for n in nodes]
+    pool_labels = [p.labels for p in pools]
+    everything = (b"\x01" * len(nodes), b"\x01" * len(pools))
+    class_of_sig = {everything: 0}
+    class_of_selector = {}
+    pod_class = np.zeros(len(pods), dtype=np.uint8)
+    for i, pod in enumerate(pods):
+        selectors = pod.selectors
+        if not selectors:
+            continue
+        items = tuple(sorted(selectors.items()))
+        c = class_of_selector.get(items)
+        if c is None:
+            sig = (bytes(_selector_matches(l, items) for l in node_labels),
+                   bytes(_selector_matches(l, items) for l in pool_labels))
+            c = class_of_sig.get(sig)
+            if c is None:
+                c = len(class_of_sig)
+                if c >= MAX_SELECTOR_CLASSES:
+                    raise ValueError("more than %d distinct node-selector match signatures are not supported"
+                                     % MAX_SELECTOR_CLASSES)
+                class_of_sig[sig] = c
+            class_of_selector[items] = c
+        pod_class[i] = c
+    node_match = np.ones(len(nodes), dtype=np.uint64)
+    pool_match = np.ones(len(pools), dtype=np.uint64)
+    for (nsig, psig), c in class_of_sig.items():
+        if c:
+            bit = np.uint64(1) << np.uint64(c)
+            node_match[np.frombuffer(nsig, dtype=np.uint8).astype(bool)] |= bit
+            pool_match[np.frombuffer(psig, dtype=np.uint8).astype(bool)] |= bit
+    return SelectorClasses(pod_class, node_match, pool_match, len(class_of_sig))
+
+
+# ------------------------------------------------------------------------------------------------
 # K0: feasibility (capacity.is_possible over the pools)
 # ------------------------------------------------------------------------------------------------
-def feasible_pods(pods, agent_pools):
-    """bool[len(pods)]: (RESOURCE_SPEC[pool.instance_type] - pod.resources).possible for some pool."""
+def feasible_pods(pods, agent_pools, classes=None):
+    """bool[len(pods)]: (RESOURCE_SPEC[pool.instance_type] - pod.resources).possible for some pool.  With `classes`
+    (selector_classes(pods, [], agent_pools)) the pool must also match the pod's nodeSelector."""
     from . import capacity
     pods = list(pods)
     if not pods:
@@ -151,7 +218,11 @@ def feasible_pods(pods, agent_pools):
     bad = _nonfinite_rows(req)       # an infinite request fits nowhere (cap - inf < 0)
     req[bad] = 0.0
     eng = get_engine()
-    mask, _ = eng.feasible_mask(eng.dev(req, torch.float64), eng.dev(unit, torch.float64))
+    if classes is not None and not classes.trivial:
+        mask, _ = eng.feasible_mask_sel(eng.dev(req, torch.float64), eng.dev(unit, torch.float64),
+                                        eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
+    else:
+        mask, _ = eng.feasible_mask(eng.dev(req, torch.float64), eng.dev(unit, torch.float64))
     out = mask.cpu().numpy().astype(bool)
     out[bad] = False
     return out
@@ -199,8 +270,9 @@ def count_running_pods(nodes, running_pods):
 # ------------------------------------------------------------------------------------------------
 # first fit over nodes (Cluster.get_pending_pods)
 # ------------------------------------------------------------------------------------------------
-def first_fit_nodes(pods, nodes):
-    """returns placed[len(pods)] (node index or -1) and mutates node.used_capacity like count_pod."""
+def first_fit_nodes(pods, nodes, classes=None):
+    """returns placed[len(pods)] (node index or -1) and mutates node.used_capacity like count_pod.  With `classes`
+    (selector_classes(pods, nodes, [])) a pod only takes a node that matches its nodeSelector."""
     pods, nodes = list(pods), list(nodes)
     placed = np.full(len(pods), -1, dtype=np.int32)
     if not pods or not nodes:
@@ -214,9 +286,16 @@ def first_fit_nodes(pods, nodes):
     req[bad] = 0.0
     eng = get_engine()
     d_used = eng.dev(used, torch.float64)
-    d_placed, _ = eng.first_fit_nodes(eng.dev(req, torch.float64),
-                                      None if not bad.any() else eng.dev(ok_idx, torch.int32),
-                                      eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used)
+    if classes is not None and not classes.trivial:
+        d_placed, _ = eng.first_fit_nodes_sel(eng.dev(req, torch.float64),
+                                              None if not bad.any() else eng.dev(ok_idx, torch.int32),
+                                              eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
+                                              eng.dev(classes.pod_class, torch.uint8),
+                                              eng.dev(classes.node_match.view(np.int64), torch.int64), classes.classes)
+    else:
+        d_placed, _ = eng.first_fit_nodes(eng.dev(req, torch.float64),
+                                          None if not bad.any() else eng.dev(ok_idx, torch.int32),
+                                          eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used)
     res = d_placed.cpu().numpy()
     if bad.any():
         placed[ok_idx] = res
@@ -249,8 +328,9 @@ def single_can_fit(node, resources):
 # ------------------------------------------------------------------------------------------------
 # fulfill_pending (bins)
 # ------------------------------------------------------------------------------------------------
-def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_provision):
-    """Scaler.fulfill_pending's packing + size arithmetic; pools already in visiting order."""
+def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_provision, classes=None):
+    """Scaler.fulfill_pending's packing + size arithmetic; pools already in visiting order.  With `classes`
+    (selector_classes(unique_pods, [], ordered_pools)) a pool only takes the pods whose nodeSelector it matches."""
     from . import capacity
     units = [capacity.RESOURCE_SPEC[pool.instance_type] for pool in ordered_pools]
     dims = Dims([p.resources for p in unique_pods] + units)
@@ -259,12 +339,14 @@ def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_pro
     _check_finite(unit, "unit capacity")
     _check_finite(req, "pending pod request")  # pending pods passed is_possible, so they are finite
     eng = get_engine()
-    res = eng.fulfill_pending(
-        eng.dev(req, torch.float64), num_listed, unit,
-        np.asarray([pool.actual_capacity for pool in ordered_pools], dtype=np.int32),
-        np.asarray([min(pool.max_size, 2 ** 31 - 1) for pool in ordered_pools], dtype=np.int32),
-        np.asarray([1 if pool.name in ignored_pool_names else 0 for pool in ordered_pools], dtype=np.uint8),
-        over_provision)
+    pools = (np.asarray([pool.actual_capacity for pool in ordered_pools], dtype=np.int32),
+             np.asarray([min(pool.max_size, 2 ** 31 - 1) for pool in ordered_pools], dtype=np.int32),
+             np.asarray([1 if pool.name in ignored_pool_names else 0 for pool in ordered_pools], dtype=np.uint8))
+    if classes is not None and not classes.trivial:
+        res = eng.fulfill_pending_sel(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
+                                      eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
+    else:
+        res = eng.fulfill_pending(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision)
     res["acc_pool"] = res["acc_pool"].cpu().numpy()
     res["bin_of"] = res["bin_of"].cpu().numpy()
     return res
