@@ -82,6 +82,7 @@ enum {
 #define ACSFIT_PODF_UNDRAINABLE 2u /* not (is_drainable() or 'kube-proxy' in name)    scaler.py:82-83 */
 /* per node flag bits */
 #define ACSFIT_NODEF_UNSCHEDULABLE 1u /* spec.unschedulable  kube.py:105 */
+#define ACSFIT_NODEF_NO_PENDING_MATCH 2u /* no pod to schedule matches the node's labels (opt-in, see node_states) */
 
 typedef struct acsfit_ctx acsfit_ctx;
 typedef void *acsfit_stream_t;
@@ -207,6 +208,10 @@ ACSFIT_API acsfit_status acsfit_fulfill_pending(acsfit_ctx *ctx, const double *r
  *   node_age [dev] N int64 seconds ((now - creation).seconds, scaler.py:78),
  *   any_pending = len(pods_to_schedule) > 0, idle_threshold [host] S int64,
  *   out_state [dev] S x N bytes.
+ * A node with ACSFIT_NODEF_NO_PENDING_MATCH is classified as if any_pending were 0: the caller sets
+ * it when no pod to schedule matches the node's nodeSelector labels, so POD_PENDING means "some
+ * pending pod could land here" (upstream ec2-autoscaler get_node_state).  A caller that never sets
+ * the bit gets the reference's "any pod to schedule" rule.  acsfit_maintain_host reads the same bits.
  */
 ACSFIT_API acsfit_status acsfit_node_states(acsfit_ctx *ctx, const int64_t *row_ptr, const int32_t *run_idx,
                                  const double *req_run, const uint8_t *flags_run,

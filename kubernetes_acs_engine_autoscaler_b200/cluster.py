@@ -54,13 +54,20 @@ class Cluster(object):
                  subscription_id, client_private_key, ca_private_key,
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
-                 over_provision=5, dry_run=False, node_selectors=None):
+                 over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
         if node_selectors is None:
             node_selectors = os.environ.get('ACSFIT_NODE_SELECTORS', '0') not in ('', '0')
         self.node_selectors = bool(node_selectors)
+        # with node selectors on, also in maintain: a node is pod-pending only when a pod to schedule matches it, so a
+        # pod pinned to one pool does not freeze scale-down in the others (opt-in; None: $ACSFIT_SELECTOR_NODE_STATES)
+        if selector_node_states is None:
+            selector_node_states = os.environ.get('ACSFIT_SELECTOR_NODE_STATES', '0') not in ('', '0')
+        elif selector_node_states and not self.node_selectors:
+            raise ValueError("selector_node_states=True needs node_selectors on")
+        self.selector_node_states = bool(selector_node_states) and self.node_selectors
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -160,7 +167,8 @@ class Cluster(object):
             resource_group=self.resource_group, nodes=all_nodes, deployments=self.deployments,
             arm_template=self.arm_template, arm_parameters=self.arm_parameters, dry_run=self.dry_run,
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
-            idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors)
+            idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
+            selector_node_states=self.selector_node_states)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [

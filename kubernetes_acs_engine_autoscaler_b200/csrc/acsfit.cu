@@ -412,12 +412,14 @@ __global__ void node_states_kernel(const int64_t *__restrict__ row_ptr, const in
             const double left = __dsub_rn(__dmul_rn(cap[d], 0.3), util[d]);
             under = under && (left >= 0.0);
         }
-        const bool unsched = node_flags[n] & ACSFIT_NODEF_UNSCHEDULABLE;
+        const uint8_t nf = node_flags[n];
+        const bool unsched = nf & ACSFIT_NODEF_UNSCHEDULABLE;
+        const bool pending = any_pending && !(nf & ACSFIT_NODEF_NO_PENDING_MATCH);
         const int64_t age = node_age[n];
         for (int s = 0; s < S; ++s) {
             uint8_t st;
             if (busy && !under) st = unsched ? ACSFIT_ST_BUSY_UNSCHEDULABLE : ACSFIT_ST_BUSY;
-            else if (any_pending && !unsched) st = ACSFIT_ST_POD_PENDING;
+            else if (pending && !unsched) st = ACSFIT_ST_POD_PENDING;
             else if (age <= idle_threshold[s] && !unsched) st = ACSFIT_ST_GRACE_PERIOD;
             else if (under && (busy || !unsched))
                 st = undrainable ? ACSFIT_ST_UNDER_UTILIZED_UNDRAINABLE : ACSFIT_ST_UNDER_UTILIZED_DRAINABLE;
@@ -538,12 +540,14 @@ node_stream_kernel(const int64_t *__restrict__ row_ptr, const int32_t *__restric
             const double left = __dsub_rn(__dmul_rn(cap[d], 0.3), acc[d]);
             under = under && (left >= 0.0);
         }
-        const bool unsched = node_flags[n] & ACSFIT_NODEF_UNSCHEDULABLE;
+        const uint8_t nf = node_flags[n];
+        const bool unsched = nf & ACSFIT_NODEF_UNSCHEDULABLE;
+        const bool pending = any_pending && !(nf & ACSFIT_NODEF_NO_PENDING_MATCH);
         const int64_t age = node_age[n];
         for (int s = 0; s < S; ++s) {
             uint8_t st;
             if (busy && !under) st = unsched ? ACSFIT_ST_BUSY_UNSCHEDULABLE : ACSFIT_ST_BUSY;
-            else if (any_pending && !unsched) st = ACSFIT_ST_POD_PENDING;
+            else if (pending && !unsched) st = ACSFIT_ST_POD_PENDING;
             else if (age <= idle_threshold[s] && !unsched) st = ACSFIT_ST_GRACE_PERIOD;
             else if (under && (busy || !unsched))
                 st = undrainable ? ACSFIT_ST_UNDER_UTILIZED_UNDRAINABLE : ACSFIT_ST_UNDER_UTILIZED_DRAINABLE;

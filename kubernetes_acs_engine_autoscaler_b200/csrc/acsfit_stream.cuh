@@ -151,11 +151,12 @@ node_stream_bulk_kernel(const int64_t *__restrict__ row_ptr, const double *__res
             under = under && (left >= 0.0);
         }
         const bool unsched = nflags & ACSFIT_NODEF_UNSCHEDULABLE;
+        const bool pending = any_pending && !(nflags & ACSFIT_NODEF_NO_PENDING_MATCH);
         const int64_t age = nage;
         for (int s = 0; s < S; ++s) {
             uint8_t st;
             if (busy && !under) st = unsched ? ACSFIT_ST_BUSY_UNSCHEDULABLE : ACSFIT_ST_BUSY;
-            else if (any_pending && !unsched) st = ACSFIT_ST_POD_PENDING;
+            else if (pending && !unsched) st = ACSFIT_ST_POD_PENDING;
             else if (age <= idle_threshold[s] && !unsched) st = ACSFIT_ST_GRACE_PERIOD;
             else if (under && (busy || !unsched))
                 st = undrainable ? ACSFIT_ST_UNDER_UTILIZED_UNDRAINABLE : ACSFIT_ST_UNDER_UTILIZED_DRAINABLE;

@@ -21,10 +21,12 @@ ACT_NONE, ACT_CORDON_DRAIN, ACT_CORDON, ACT_UNCORDON, ACT_SCALE_IN = range(5)
 
 class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
-                 deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False):
+                 deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
+                 selector_node_states=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
+        self.selector_node_states = selector_node_states
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)
@@ -110,7 +112,8 @@ class EngineScaler(Scaler):
         delete_queue = []
         if nodes:
             lists = [pods_by_node.get(node.name, []) for node in nodes]
-            state_dev = snapshot.node_states(nodes, lists, bool(pods_to_schedule), self.idle_threshold)
+            state_dev = snapshot.node_states(nodes, lists, bool(pods_to_schedule), self.idle_threshold,
+                                             no_match=self.no_pending_match(nodes, pods_to_schedule))
             states, actions = snapshot.maintain_actions(state_dev, node_pool, budget0, [1] * len(budget0),
                                                         self.dry_run)
             info = logger.isEnabledFor(logging.INFO)  # (formatted eagerly, as upstream: skipped when nobody listens)

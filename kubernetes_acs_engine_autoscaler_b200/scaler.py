@@ -62,6 +62,8 @@ class Scaler(object):
         self.scalable_pools = None
         self.ignored_pool_names = {}
         self.node_selectors = False  # honour the pods' nodeSelectors (Cluster(node_selectors=...))
+        # POD_PENDING only when a pod to schedule matches the node (Cluster(selector_node_states=...))
+        self.selector_node_states = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -69,10 +71,18 @@ class Scaler(object):
     def scale_pools(self, pool_sizes):
         raise NotImplementedError()
 
+    def no_pending_match(self, nodes, pods_to_schedule):
+        """bool[len(nodes)] for snapshot.node_states(no_match=...): the nodes no pod to schedule matches, or None
+        when every node keeps the reference's "any pod to schedule" rule (the switch is off, or nothing is pending)."""
+        if not self.selector_node_states or not pods_to_schedule:
+            return None
+        return ~snapshot.pending_match(pods_to_schedule, nodes)
+
     def get_node_state(self, node, node_pods, pods_to_schedule):
         """ClusterNodeState of one node (scaler.py:61-114): a one-node launch of the idle scan.
         EngineScaler.maintain classifies all nodes in a single launch instead."""
-        code = snapshot.node_states([node], [list(node_pods)], bool(pods_to_schedule), self.idle_threshold)
+        code = snapshot.node_states([node], [list(node_pods)], bool(pods_to_schedule), self.idle_threshold,
+                                    no_match=self.no_pending_match([node], pods_to_schedule))
         return STATE_NAMES[int(code.cpu().numpy()[0])]
 
     def fulfill_pending(self, pods):

@@ -198,6 +198,52 @@ def selector_classes(pods, nodes, pools):
     return SelectorClasses(pod_class, node_match, pool_match, len(class_of_sig))
 
 
+def pending_match(pods, nodes):
+    """bool[N]: some pod of `pods` matches node n (KubeNode.is_match).  All True when a pod has no selector.
+
+    Maintain asks this of every node of the scalable pools (up to 10^6), so selectors are not evaluated node by node.
+    Each label key any selector uses is read once per node and its values are numbered (a missing label reads as None,
+    as labels.get does in is_match); the nodes are grouped by their projection, the tuple of those numbers; and each
+    distinct selector is evaluated once per distinct projection, vectorised over the projections."""
+    nodes = list(nodes)
+    selectors = {}
+    for pod in pods:
+        if not pod.selectors:
+            return np.ones(len(nodes), dtype=bool)
+        selectors.setdefault(tuple(sorted(pod.selectors.items())), None)
+    if not selectors or not nodes:
+        return np.zeros(len(nodes), dtype=bool)
+    keys = sorted({key for items in selectors for key, _ in items})
+    labels = [n.selectors for n in nodes]
+    code_of, codes = [], []  # per key: {value: number}, and the number of every node's value
+    group, bound = np.zeros(len(nodes), dtype=np.int64), 1  # mixed-radix projection number so far, and its range
+    for key in keys:
+        values = [l.get(key) for l in labels]
+        code = {v: i for i, v in enumerate(dict.fromkeys(values))}
+        code_of.append(code)
+        codes.append(np.fromiter(map(code.__getitem__, values), dtype=np.int64, count=len(values)))
+        if bound * len(code) >= 1 << 62:  # renumber densely (below N) before the number could overflow
+            _, group = np.unique(group, return_inverse=True)
+            group, bound = group.reshape(-1), len(nodes)
+        group, bound = group * len(code) + codes[-1], bound * len(code)
+    _, first, group = np.unique(group, return_index=True, return_inverse=True)
+    group = group.reshape(-1)
+    proj = np.stack([c[first] for c in codes], axis=1)  # [distinct projections, keys]
+    column = {key: k for k, key in enumerate(keys)}
+    hit = np.zeros(len(first), dtype=bool)
+    for items in selectors:
+        match = ~hit
+        for key, value in items:
+            k = column[key]
+            c = code_of[k].get(value)
+            if c is None:  # no node carries this value (or, for None, lacks the key)
+                match[:] = False
+                break
+            match &= proj[:, k] == c
+        hit |= match
+    return hit[group]
+
+
 # ------------------------------------------------------------------------------------------------
 # K0: feasibility (capacity.is_possible over the pools)
 # ------------------------------------------------------------------------------------------------
@@ -356,7 +402,7 @@ def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_pro
 # idle scan + maintain decisions
 # ------------------------------------------------------------------------------------------------
 POD_BUSY, POD_UNDRAINABLE = 1, 2
-NODE_UNSCHEDULABLE = 1
+NODE_UNSCHEDULABLE, NODE_NO_PENDING_MATCH = 1, 2
 
 
 def pod_flags(pod, now_by_tz=None):
@@ -402,8 +448,10 @@ def node_age_seconds(node, now_by_tz=None):
     return (now - node.creation_time).seconds
 
 
-def node_states(nodes, pods_lists, any_pending, idle_threshold):
-    """state code per node (include/acsfit.h ACSFIT_ST_*); pods_lists[n] = the node's pods in order."""
+def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None):
+    """state code per node (include/acsfit.h ACSFIT_ST_*); pods_lists[n] = the node's pods in order.  `no_match`
+    (bool[N], optional): nodes no pod to schedule matches (~pending_match); they are classified as if there were no
+    pod to schedule (ACSFIT_NODEF_NO_PENDING_MATCH)."""
     nodes = list(nodes)
     if not nodes:
         return np.zeros(0, dtype=np.uint8)
@@ -419,6 +467,8 @@ def node_states(nodes, pods_lists, any_pending, idle_threshold):
     flags = np.asarray([pod_flags(p, clock) for p in flat], dtype=np.uint8)
     cap, node_type = _node_types(nodes, dims)
     node_flags = np.asarray([NODE_UNSCHEDULABLE if n.unschedulable else 0 for n in nodes], dtype=np.uint8)
+    if no_match is not None:
+        node_flags |= np.where(np.asarray(no_match, dtype=bool), np.uint8(NODE_NO_PENDING_MATCH), np.uint8(0))
     age = np.asarray([node_age_seconds(n, clock) for n in nodes], dtype=np.int64)
     eng = get_engine()
     st = eng.node_states(eng.dev(row_ptr, torch.int64),
