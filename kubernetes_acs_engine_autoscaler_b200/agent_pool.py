@@ -1,6 +1,7 @@
 """Agent pool = name + instance type + its nodes (mirror of reference autoscaler/agent_pool.py)."""
 import logging
 
+from . import kube
 from .capacity import get_capacity_for_instance_type
 
 logger = logging.getLogger('autoscaler.agent_pool')
@@ -43,6 +44,17 @@ class AgentPool(object):
         common['agentpool'] = self.name
         common['beta.kubernetes.io/instance-type'] = self.instance_type
         return common
+
+    @property
+    def taints(self):
+        """the blocking taints a new node of this pool will carry, for matching tolerations: every blocking,
+        non-lifecycle taint (kube.blocking_taints) all current nodes carry with the same key, value and effect, as
+        (key, value, effect) tuples in sorted order.  An empty pool has none."""
+        common = None
+        for node in self.nodes:
+            mine = kube.blocking_taints(node.taints)
+            common = mine if common is None else common & mine
+        return sorted(common or ())
 
     def reclaim_unschedulable_nodes(self, new_desired_capacity):
         """uncordon just enough of our own cordoned nodes before asking for new VMs

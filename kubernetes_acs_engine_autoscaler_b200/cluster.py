@@ -54,7 +54,8 @@ class Cluster(object):
                  subscription_id, client_private_key, ca_private_key,
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
-                 over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None):
+                 over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
+                 node_taints=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -68,6 +69,14 @@ class Cluster(object):
         elif selector_node_states and not self.node_selectors:
             raise ValueError("selector_node_states=True needs node_selectors on")
         self.selector_node_states = bool(selector_node_states) and self.node_selectors
+        # with node selectors on, a pod matches a node or pool only when it also tolerates every blocking taint there,
+        # so a tainted (e.g. GPU) pool neither absorbs nor holds back the pods it would refuse (opt-in; None:
+        # $ACSFIT_NODE_TAINTS)
+        if node_taints is None:
+            node_taints = os.environ.get('ACSFIT_NODE_TAINTS', '0') not in ('', '0')
+        elif node_taints and not self.node_selectors:
+            raise ValueError("node_taints=True needs node_selectors on")
+        self.node_taints = bool(node_taints) and self.node_selectors
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -168,7 +177,7 @@ class Cluster(object):
             arm_template=self.arm_template, arm_parameters=self.arm_parameters, dry_run=self.dry_run,
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
             idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
-            selector_node_states=self.selector_node_states)
+            selector_node_states=self.selector_node_states, node_taints=self.node_taints)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [
@@ -196,7 +205,9 @@ class Cluster(object):
         """sequential first fit of the pods over the nodes (cluster.py:184-204); placed pods are
         counted into node.used_capacity, the rest are returned in order."""
         pods, nodes = list(pods), list(nodes)
-        classes = snapshot.selector_classes(pods, nodes, []) if self.node_selectors else None
+        classes = None
+        if self.node_selectors:
+            classes = snapshot.selector_classes(pods, nodes, [], taints=self.node_taints)
         placed = snapshot.first_fit_nodes(pods, nodes, classes=classes)
         detail = len(pods) <= LOG_DETAIL_LIMIT
         pending_pods = []
@@ -226,19 +237,28 @@ class Cluster(object):
         pending_unassigned_pods = [p for p in pods if p.status == KubePodStatus.PENDING and (not p.node_name)]
         classes = None
         if self.node_selectors:
-            classes = snapshot.selector_classes(pending_unassigned_pods, [], agent_pools)
+            classes = snapshot.selector_classes(pending_unassigned_pods, [], agent_pools, taints=self.node_taints)
         feasible = snapshot.feasible_pods(pending_unassigned_pods, agent_pools, classes=classes)
         unmatched = set()  # rejected only because no pool that would fit matches the node selector
+        untolerated = set()  # some pool that would fit matches the selector, but each has a taint the pod does not tolerate
         if classes is not None and not classes.trivial:
             rejected = [p for p, ok, c in zip(pending_unassigned_pods, feasible, classes.pod_class) if not ok and c]
             if rejected:
                 fits = snapshot.feasible_pods(rejected, agent_pools)
                 unmatched = {id(p) for p, ok in zip(rejected, fits) if ok}
+            if unmatched and self.node_taints:
+                fitting = [p for p in rejected if id(p) in unmatched]
+                selected = snapshot.feasible_pods(fitting, agent_pools,
+                                                  classes=snapshot.selector_classes(fitting, [], agent_pools))
+                untolerated = {id(p) for p, ok in zip(fitting, selected) if ok}
         pods_to_schedule = []
         warn = logger.isEnabledFor(logging.WARNING)  # (the message is formatted eagerly, as upstream: skip it when nobody listens)
         for pod, ok in zip(pending_unassigned_pods, feasible):
             if ok:
                 pods_to_schedule.append(pod)
+            elif warn and id(pod) in untolerated:
+                logger.warning("Pending pod %s cannot fit: every agent pool that would fit it and matches its node "
+                               "selector has a taint it does not tolerate. Scheduling skipped." % pod.name)
             elif warn and id(pod) in unmatched:
                 logger.warning("Pending pod %s cannot fit: no agent pool matches its node selector %s. "
                                "Scheduling skipped." % (pod.name, pod.selectors))

@@ -10,6 +10,7 @@ import datetime
 import json
 import logging
 import os
+from collections.abc import Mapping
 
 from . import utils
 
@@ -23,6 +24,62 @@ except ImportError:
     _hostfast = None
 
 _CORDON_LABEL = 'openai/cordoned-by-autoscaler'
+
+# taint effects that keep a pod which does not tolerate them off a node (PreferNoSchedule is only a preference)
+BLOCKING_EFFECTS = ('NoSchedule', 'NoExecute')
+# node-lifecycle taints (unschedulable, not-ready, unreachable, uninitialized) are not honoured: cordoning is modelled
+# by spec.unschedulable, and a node booting from this autoscaler's own scale-up carries not-ready / uninitialized for
+# a while -- honouring those would make the next tick scale up again for the same pods
+LIFECYCLE_TAINT_PREFIXES = ('node.kubernetes.io/', 'node.alpha.kubernetes.io/', 'node.cloudprovider.kubernetes.io/')
+
+
+def _field(entry, key):
+    value = entry.get(key)
+    return '' if value is None else value
+
+
+def _entries(value, what, owner):
+    """spec.taints / spec.tolerations as a list of mappings ([] when absent); ValueError naming the owner otherwise"""
+    if value is None:
+        return []
+    if not isinstance(value, list) or not all(type(e) is dict or isinstance(e, Mapping) for e in value):
+        raise ValueError("malformed %s of %s: expected a list of mappings, got %r" % (what, owner, value))
+    return value
+
+
+def blocking_taints(taints):
+    """frozenset of (key, value, effect) of the taints that block scheduling: effect NoSchedule or NoExecute, and not
+    a node-lifecycle taint (LIFECYCLE_TAINT_PREFIXES)"""
+    out = set()
+    for t in taints:
+        key, effect = _field(t, 'key'), _field(t, 'effect')
+        if effect in BLOCKING_EFFECTS and not key.startswith(LIFECYCLE_TAINT_PREFIXES):
+            out.add((key, _field(t, 'value'), effect))
+    return frozenset(out)
+
+
+def tolerates(tolerations, taint):
+    """some toleration tolerates the taint (Kubernetes' Toleration.ToleratesTaint): a non-empty effect must equal the
+    taint's, a non-empty key must equal the taint's (an empty key matches every key); operator Exists matches any value,
+    Equal or an empty operator needs equal values (a missing value reads as ''), any other operator tolerates nothing.
+    tolerationSeconds is ignored.  `taint` is a mapping or a (key, value, effect) tuple."""
+    if not isinstance(taint, Mapping):
+        taint = dict(zip(('key', 'value', 'effect'), taint))
+    key, value, effect = _field(taint, 'key'), _field(taint, 'value'), _field(taint, 'effect')
+    for t in tolerations:
+        if _field(t, 'effect') and _field(t, 'effect') != effect:
+            continue
+        if _field(t, 'key') and _field(t, 'key') != key:
+            continue
+        op = _field(t, 'operator')
+        if op == 'Exists' or (op in ('', 'Equal') and _field(t, 'value') == value):
+            return True
+    return False
+
+
+def tolerates_all(tolerations, taints):
+    """the pod with these tolerations may be scheduled past every one of `taints` (blocking_taints tuples)"""
+    return all(tolerates(tolerations, t) for t in taints)
 
 
 class KubePodStatus(object):
@@ -161,6 +218,12 @@ class KubePod(object):
             _CREATED_BY_MEMO[text] = decoded
         return decoded
 
+    @property
+    def tolerations(self):
+        """spec.tolerations ([] when absent); read on use, so pods built attribute by attribute (make_pods) have it too.
+        ValueError when it is not a list of mappings."""
+        return _entries(self.original.obj['spec'].get('tolerations'), 'spec.tolerations', 'pod %s' % self)
+
     def is_mirrored(self):
         daemonset = self._created_by().get('reference', {}).get('kind') == 'DaemonSet'
         return daemonset or self.annotations.get('kubernetes.io/config.mirror')
@@ -222,6 +285,11 @@ class KubeNode(object):
         self.unschedulable = node.obj['spec'].get('unschedulable', False)
         self.creation_time = utils.parse_time(meta['creationTimestamp'])
         self.instance_index = utils.get_instance_index(node)
+
+    @property
+    def taints(self):
+        """spec.taints as listed ([] when absent); read on use.  ValueError when it is not a list of mappings."""
+        return _entries(self.original.obj['spec'].get('taints'), 'spec.taints', 'node %s' % self)
 
     def _get_instance_data(self):
         labels = self.original.obj['metadata']['labels']

@@ -64,6 +64,9 @@ class Scaler(object):
         self.node_selectors = False  # honour the pods' nodeSelectors (Cluster(node_selectors=...))
         # POD_PENDING only when a pod to schedule matches the node (Cluster(selector_node_states=...))
         self.selector_node_states = False
+        # with node selectors: a pod matches a node or pool only when it also tolerates its blocking taints
+        # (Cluster(node_taints=...))
+        self.node_taints = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -76,7 +79,7 @@ class Scaler(object):
         when every node keeps the reference's "any pod to schedule" rule (the switch is off, or nothing is pending)."""
         if not self.selector_node_states or not pods_to_schedule:
             return None
-        return ~snapshot.pending_match(pods_to_schedule, nodes)
+        return ~snapshot.pending_match(pods_to_schedule, nodes, taints=self.node_taints)
 
     def get_node_state(self, node, node_pods, pods_to_schedule):
         """ClusterNodeState of one node (scaler.py:61-114): a one-node launch of the idle scan.
@@ -92,7 +95,9 @@ class Scaler(object):
         # occurrence, but num_unaccounted starts at len(pods) (scaler.py:119-120)
         unique = list(dict((p, False) for p in pods).keys())
         ordered_pools = capacity.order_by_cost_asc(self.agent_pools)
-        classes = snapshot.selector_classes(unique, [], ordered_pools) if self.node_selectors else None
+        classes = None
+        if self.node_selectors:
+            classes = snapshot.selector_classes(unique, [], ordered_pools, taints=self.node_taints)
         res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision,
                                classes=classes)
 

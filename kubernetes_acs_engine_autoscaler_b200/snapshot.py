@@ -12,6 +12,7 @@ is padded with zero columns to 2/4/8/16 for the first-fit kernels.
 import numpy as np
 import torch
 
+from . import kube
 from .engine import Engine, padded_dims
 from .kube import _hostfast
 
@@ -140,7 +141,8 @@ MAX_SELECTOR_CLASSES = 64
 
 class SelectorClasses(object):
     """pod_class uint8[P], node_match uint64[N], pool_match uint64[T] (in the order the pools were given) and the
-    number of classes.  Bit c of a mask is set when the node / pool matches the selectors of class c."""
+    number of classes.  Bit c of a mask is set when the node / pool matches the selectors (and, with taints, the
+    tolerations) of class c."""
 
     def __init__(self, pod_class, node_match, pool_match, classes):
         self.pod_class = pod_class
@@ -158,90 +160,148 @@ def _selector_matches(labels, items):
     return all(labels.get(key) == value for key, value in items)  # KubeNode.is_match
 
 
-def selector_classes(pods, nodes, pools):
+def _toleration_items(tolerations):
+    """a hashable key of a toleration list (two pods with equal keys tolerate the same taints)"""
+    return tuple(tuple(sorted(t.items())) for t in tolerations)
+
+
+class _Projection(object):
+    """the nodes grouped by everything a match can see, so that a match is evaluated once per distinct projection,
+    vectorised over the projections, instead of once per node.  Each label key in `keys` is read once per node and its
+    values are numbered (a missing label reads as None, as labels.get does in is_match); with `taints`, the node's
+    blocking-taint set (kube.blocking_taints) is numbered as one more column.  `group[n]` is node n's projection."""
+
+    def __init__(self, nodes, keys, taints):
+        codes, self.code_of = [], []  # the number of every node's value per column; per label key: {value: number}
+        labels = [n.selectors for n in nodes] if keys else []
+        for key in keys:
+            values = [l.get(key) for l in labels]
+            code = {v: i for i, v in enumerate(dict.fromkeys(values))}
+            self.code_of.append(code)
+            codes.append(np.fromiter(map(code.__getitem__, values), dtype=np.int64, count=len(values)))
+        self.taint_sets = []
+        if taints:
+            sets = [kube.blocking_taints(n.taints) for n in nodes]
+            code = {s: i for i, s in enumerate(dict.fromkeys(sets))}
+            self.taint_sets = list(code)
+            codes.append(np.fromiter(map(code.__getitem__, sets), dtype=np.int64, count=len(sets)))
+        group, bound = np.zeros(len(nodes), dtype=np.int64), 1  # mixed-radix projection number so far, and its range
+        for c in codes:
+            radix = int(c.max()) + 1 if len(c) else 1
+            if bound * radix >= 1 << 62:  # renumber densely (below N) before the number could overflow
+                _, group = np.unique(group, return_inverse=True)
+                group, bound = group.reshape(-1), len(nodes)
+            group, bound = group * radix + c, bound * radix
+        _, first, group = np.unique(group, return_index=True, return_inverse=True)
+        self.group = group.reshape(-1)
+        self.proj = np.stack([c[first] for c in codes], axis=1) if codes else np.zeros((len(first), 0), np.int64)
+        self.column = {key: k for k, key in enumerate(keys)}
+
+    def selector(self, items):
+        """bool[projections]: the labels match the selector `items` (KubeNode.is_match)"""
+        match = np.ones(len(self.proj), dtype=bool)
+        for key, value in items:
+            k = self.column[key]
+            c = self.code_of[k].get(value)
+            if c is None:  # no node carries this value (or, for None, lacks the key)
+                match[:] = False
+                break
+            match &= self.proj[:, k] == c
+        return match
+
+    def tolerated(self, tolerations):
+        """bool[projections]: a pod with these tolerations tolerates every blocking taint (needs taints=True)"""
+        ok = np.fromiter((kube.tolerates_all(tolerations, s) for s in self.taint_sets), dtype=bool,
+                         count=len(self.taint_sets))
+        return ok[self.proj[:, -1]]
+
+
+def _match_keys(pods, taints):
+    """the distinct (selector items, toleration items) of the pods in first-occurrence order with one toleration list
+    each, and every pod's index into them.  Without taints a pod without a selector gets -1 (it matches everything)."""
+    index, distinct = {}, []
+    of_pod = np.full(len(pods), -1, dtype=np.int64)
+    for i, pod in enumerate(pods):
+        selectors = pod.selectors
+        tolerations = pod.tolerations if taints else ()
+        if not selectors and not taints:
+            continue
+        key = (tuple(sorted(selectors.items())) if selectors else (),
+               _toleration_items(tolerations) if tolerations else ())
+        j = index.get(key)
+        if j is None:
+            j = index[key] = len(distinct)
+            distinct.append((key[0], tolerations))
+        of_pod[i] = j
+    return distinct, of_pod
+
+
+def selector_classes(pods, nodes, pools, taints=False):
     """map every distinct match signature (set of matching nodes, set of matching pools) of the pods' nodeSelectors
     to a class number.  Class 0 is "no selector": it matches everything, so a selector that matches every node and
     every pool shares it.  Pods whose selectors match the same nodes and pools share a class.  A pool matches with
-    the labels a new node of it would carry (AgentPool.labels).  Raises ValueError above 64 classes."""
+    the labels a new node of it would carry (AgentPool.labels).  Raises ValueError above 64 classes.
+
+    With `taints`, a pod matches a node or pool when its selector matches AND it tolerates every blocking taint there
+    (kube.blocking_taints of KubeNode.taints, AgentPool.taints; KubePod.tolerations).  Class 0 keeps its meaning
+    (matches every node and pool); it may then have no pod.  Without `taints`, taints and tolerations are never read.
+    Each distinct (selector, tolerations) is evaluated once per distinct node projection (_Projection)."""
     pods, nodes, pools = list(pods), list(nodes), list(pools)
-    node_labels = [n.selectors for n in nodes]
+    distinct, of_pod = _match_keys(pods, taints)
+    if not distinct:
+        return SelectorClasses(np.zeros(len(pods), dtype=np.uint8), np.ones(len(nodes), dtype=np.uint64),
+                               np.ones(len(pools), dtype=np.uint64), 1)
+    proj = _Projection(nodes, sorted({key for items, _ in distinct for key, _ in items}), taints)
     pool_labels = [p.labels for p in pools]
-    everything = (b"\x01" * len(nodes), b"\x01" * len(pools))
+    pool_taints = [p.taints for p in pools] if taints else [()] * len(pools)
+    everything = (b"\x01" * len(proj.proj), b"\x01" * len(pools))
     class_of_sig = {everything: 0}
-    class_of_selector = {}
-    pod_class = np.zeros(len(pods), dtype=np.uint8)
-    for i, pod in enumerate(pods):
-        selectors = pod.selectors
-        if not selectors:
-            continue
-        items = tuple(sorted(selectors.items()))
-        c = class_of_selector.get(items)
+    class_of_key = np.zeros(len(distinct) + 1, dtype=np.uint8)  # the last entry (index -1) is class 0
+    for j, (items, tolerations) in enumerate(distinct):
+        nmatch = proj.selector(items)
+        if taints:
+            nmatch &= proj.tolerated(tolerations)
+        sig = (nmatch.tobytes(), bytes(_selector_matches(l, items) and kube.tolerates_all(tolerations, t)
+                                       for l, t in zip(pool_labels, pool_taints)))
+        c = class_of_sig.get(sig)
         if c is None:
-            sig = (bytes(_selector_matches(l, items) for l in node_labels),
-                   bytes(_selector_matches(l, items) for l in pool_labels))
-            c = class_of_sig.get(sig)
-            if c is None:
-                c = len(class_of_sig)
-                if c >= MAX_SELECTOR_CLASSES:
-                    raise ValueError("more than %d distinct node-selector match signatures are not supported"
-                                     % MAX_SELECTOR_CLASSES)
-                class_of_sig[sig] = c
-            class_of_selector[items] = c
-        pod_class[i] = c
-    node_match = np.ones(len(nodes), dtype=np.uint64)
+            c = len(class_of_sig)
+            if c >= MAX_SELECTOR_CLASSES:
+                raise ValueError("more than %d distinct node-selector match signatures are not supported"
+                                 % MAX_SELECTOR_CLASSES)
+            class_of_sig[sig] = c
+        class_of_key[j] = c
+    node_match = np.ones(len(proj.proj), dtype=np.uint64)
     pool_match = np.ones(len(pools), dtype=np.uint64)
     for (nsig, psig), c in class_of_sig.items():
         if c:
             bit = np.uint64(1) << np.uint64(c)
             node_match[np.frombuffer(nsig, dtype=np.uint8).astype(bool)] |= bit
             pool_match[np.frombuffer(psig, dtype=np.uint8).astype(bool)] |= bit
-    return SelectorClasses(pod_class, node_match, pool_match, len(class_of_sig))
+    return SelectorClasses(class_of_key[of_pod], node_match[proj.group], pool_match, len(class_of_sig))
 
 
-def pending_match(pods, nodes):
-    """bool[N]: some pod of `pods` matches node n (KubeNode.is_match).  All True when a pod has no selector.
+def pending_match(pods, nodes, taints=False):
+    """bool[N]: some pod of `pods` matches node n (KubeNode.is_match).  All True when a pod has no selector.  With
+    `taints` a pod matches a node when its selector matches AND it tolerates the node's blocking taints: a pod without
+    a selector then matches only the nodes whose blocking taints it tolerates.
 
-    Maintain asks this of every node of the scalable pools (up to 10^6), so selectors are not evaluated node by node.
-    Each label key any selector uses is read once per node and its values are numbered (a missing label reads as None,
-    as labels.get does in is_match); the nodes are grouped by their projection, the tuple of those numbers; and each
-    distinct selector is evaluated once per distinct projection, vectorised over the projections."""
+    Maintain asks this of every node of the scalable pools (up to 10^6), so matches are not evaluated node by node:
+    each distinct (selector, tolerations) is evaluated once per distinct node projection (_Projection)."""
     nodes = list(nodes)
-    selectors = {}
-    for pod in pods:
-        if not pod.selectors:
-            return np.ones(len(nodes), dtype=bool)
-        selectors.setdefault(tuple(sorted(pod.selectors.items())), None)
-    if not selectors or not nodes:
+    if not taints and any(not pod.selectors for pod in pods):
+        return np.ones(len(nodes), dtype=bool)
+    distinct, _ = _match_keys(pods, taints)
+    if not distinct or not nodes:
         return np.zeros(len(nodes), dtype=bool)
-    keys = sorted({key for items in selectors for key, _ in items})
-    labels = [n.selectors for n in nodes]
-    code_of, codes = [], []  # per key: {value: number}, and the number of every node's value
-    group, bound = np.zeros(len(nodes), dtype=np.int64), 1  # mixed-radix projection number so far, and its range
-    for key in keys:
-        values = [l.get(key) for l in labels]
-        code = {v: i for i, v in enumerate(dict.fromkeys(values))}
-        code_of.append(code)
-        codes.append(np.fromiter(map(code.__getitem__, values), dtype=np.int64, count=len(values)))
-        if bound * len(code) >= 1 << 62:  # renumber densely (below N) before the number could overflow
-            _, group = np.unique(group, return_inverse=True)
-            group, bound = group.reshape(-1), len(nodes)
-        group, bound = group * len(code) + codes[-1], bound * len(code)
-    _, first, group = np.unique(group, return_index=True, return_inverse=True)
-    group = group.reshape(-1)
-    proj = np.stack([c[first] for c in codes], axis=1)  # [distinct projections, keys]
-    column = {key: k for k, key in enumerate(keys)}
-    hit = np.zeros(len(first), dtype=bool)
-    for items in selectors:
-        match = ~hit
-        for key, value in items:
-            k = column[key]
-            c = code_of[k].get(value)
-            if c is None:  # no node carries this value (or, for None, lacks the key)
-                match[:] = False
-                break
-            match &= proj[:, k] == c
+    proj = _Projection(nodes, sorted({key for items, _ in distinct for key, _ in items}), taints)
+    hit = np.zeros(len(proj.proj), dtype=bool)
+    for items, tolerations in distinct:
+        match = proj.selector(items)
+        if taints:
+            match &= proj.tolerated(tolerations)
         hit |= match
-    return hit[group]
+    return hit[proj.group]
 
 
 # ------------------------------------------------------------------------------------------------
