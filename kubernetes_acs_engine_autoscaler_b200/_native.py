@@ -58,6 +58,11 @@ SIGNATURES = {
     "acsfit_scale_up_sel_host": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
                                          c_vp, c_int, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                          c_vp]),
+    # pod anti-affinity: the arguments of the _sel form (sel may be NULL) plus a `const acsfit_anti_affinity *`
+    "acsfit_first_fit_nodes_aa": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp]),
+    "acsfit_fulfill_pending_aa": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
+                                          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
 }
 
 
@@ -65,6 +70,12 @@ class Selectors(ctypes.Structure):
     """struct acsfit_selectors (include/acsfit.h)"""
     _fields_ = [("pod_class", c_vp), ("node_match", c_vp), ("pool_match_all", c_vp),
                 ("pool_match_ordered", c_vp), ("classes", c_int)]
+
+
+class AntiAffinity(ctypes.Structure):
+    """struct acsfit_anti_affinity (include/acsfit.h)"""
+    _fields_ = [("pod_carries", c_vp), ("pod_matches", c_vp), ("node_carries", c_vp), ("node_matches", c_vp)]
+
 
 # one record of acsfit_last_launches (ACSFIT_LAUNCH_FIELDS ints), field names in order
 LAUNCH_FIELDS = ("pass", "chained", "D", "RW", "prune", "form", "Tn", "stages", "resident", "pool", "bin_base",

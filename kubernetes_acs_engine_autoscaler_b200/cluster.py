@@ -55,7 +55,7 @@ class Cluster(object):
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
-                 node_taints=None):
+                 node_taints=None, pod_anti_affinity=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -77,6 +77,12 @@ class Cluster(object):
         elif node_taints and not self.node_selectors:
             raise ValueError("node_taints=True needs node_selectors on")
         self.node_taints = bool(node_taints) and self.node_selectors
+        # honour required pod anti-affinity with topologyKey kubernetes.io/hostname in first fit and bin packing, so that
+        # replicas which avoid each other are not simulated onto one node (opt-in; None: $ACSFIT_POD_ANTI_AFFINITY).
+        # Independent of node_selectors; with both on, the node pass uses both.
+        if pod_anti_affinity is None:
+            pod_anti_affinity = os.environ.get('ACSFIT_POD_ANTI_AFFINITY', '0') not in ('', '0')
+        self.pod_anti_affinity = bool(pod_anti_affinity)
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -177,7 +183,8 @@ class Cluster(object):
             arm_template=self.arm_template, arm_parameters=self.arm_parameters, dry_run=self.dry_run,
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
             idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
-            selector_node_states=self.selector_node_states, node_taints=self.node_taints)
+            selector_node_states=self.selector_node_states, node_taints=self.node_taints,
+            pod_anti_affinity=self.pod_anti_affinity)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [
@@ -193,7 +200,7 @@ class Cluster(object):
 
         if self.scale_up:
             logger.info("++++ Scaling Up Begins ++++++")
-            self.scale(pods_to_schedule, all_nodes, scaler)
+            self.scale(pods_to_schedule, all_nodes, scaler, running_pods=running_or_pending_assigned_pods)
             logger.info("++++ Scaling Up Ends ++++++")
         if self.maintainance:
             logger.info("++++ Maintenance Begins ++++++")
@@ -201,14 +208,21 @@ class Cluster(object):
             logger.info("++++ Maintenance Ends ++++++")
         return True
 
-    def get_pending_pods(self, pods, nodes):
+    def get_pending_pods(self, pods, nodes, running_pods=None):
         """sequential first fit of the pods over the nodes (cluster.py:184-204); placed pods are
-        counted into node.used_capacity, the rest are returned in order."""
+        counted into node.used_capacity, the rest are returned in order.
+
+        With pod anti-affinity on, `running_pods` are the pods already on the nodes (the tick's running or assigned
+        pending pods, which scale() passes): their terms block pods, and pods' terms block them.  Without it, only the
+        pods this call places count."""
         pods, nodes = list(pods), list(nodes)
         classes = None
         if self.node_selectors:
             classes = snapshot.selector_classes(pods, nodes, [], taints=self.node_taints)
-        placed = snapshot.first_fit_nodes(pods, nodes, classes=classes)
+        anti_affinity = None
+        if self.pod_anti_affinity:
+            anti_affinity = snapshot.anti_affinity(pods, nodes, running_pods or [])
+        placed = snapshot.first_fit_nodes(pods, nodes, classes=classes, anti_affinity=anti_affinity)
         detail = len(pods) <= LOG_DETAIL_LIMIT
         pending_pods = []
         for i, pod in enumerate(pods):
@@ -224,10 +238,10 @@ class Cluster(object):
                 logger.debug(pod.name)
         return pending_pods
 
-    def scale(self, pods_to_schedule, nodes, scaler):
+    def scale(self, pods_to_schedule, nodes, scaler, running_pods=None):
         logger.info("Nodes: {}".format(len(nodes)))
         logger.info("To schedule: {}".format(len(pods_to_schedule)))
-        pending_pods = self.get_pending_pods(pods_to_schedule, nodes)
+        pending_pods = self.get_pending_pods(pods_to_schedule, nodes, running_pods=running_pods)
         if len(pending_pods) > 0:
             scaler.fulfill_pending(pending_pods)
 

@@ -1139,23 +1139,24 @@ static acsfit_status launch_stream(acsfit_ctx *ctx, const PipelineParams &pp, in
 }
 
 constexpr int kOneCtaSmemKb = 116;  // more than half of the 227 KB an SM offers: a second CTA cannot be resident
-// SEL: the node-selector form of a node pass (barrier form only: it ignores the "stream" knob)
-template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false>
+// SEL: the node-selector form of a node pass, AA: the anti-affinity form of a node or bin pass (barrier form only:
+// both ignore the "stream" knob)
+template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false, bool AA = false>
 static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
-    if constexpr (RW > 0 && D <= 8 && !PRUNE && !SEL) {
+    if constexpr (RW > 0 && D <= 8 && !PRUNE && !SEL && !AA) {
         if (stream_form_ok(ctx, D, RW, pp.Tn)) return launch_stream<D, BINS, RW>(ctx, pp, stages, st, resident);
     }
     constexpr int NT = stage_threads(D, BINS);
-    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL>::bytes(pp.Tn);
+    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL, AA>::bytes(pp.Tn);
     // D >= 8: ONE stage CTA per SM.  Whether two fit is an accident of the register allocation (the bins kernel has
     // been compiled to 128 and to 237 registers by neighbouring source revisions); at c3 a second CTA on the
     // frontier's SM costs the placement chain more than the extra resident stages give back.
     if (D >= 8) smem = std::max(smem, (size_t)kOneCtaSmemKb * 1024);
     if (ctx->smem_floor_kb > 0) smem = std::max(smem, (size_t)ctx->smem_floor_kb * 1024);  // occupancy knob
-    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL>;
+    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL, AA>;
     if (resident) {  // only asked: how many stages does the GPU hold at once?  (cached: the query costs ~10 us)
-        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0), RW, pp.Tn);
+        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0) | (AA ? 8 : 0), RW, pp.Tn);
         auto it = ctx->resident_cache.find(key);
         if (it == ctx->resident_cache.end()) {
             int per_sm = 0;
@@ -1170,7 +1171,7 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     PipelineParams q = pp;
     // more stages than the GPU holds at once: several waves, each streaming the whole pod list (see the kernel's publish)
     int held = 0;
-    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL>(ctx, pp, stages, st, &held)));
+    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA>(ctx, pp, stages, st, &held)));
     q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
     q.prof = (ctx->prof_dev && stages <= kProfStages) ? ctx->prof_dev : nullptr;
     if (q.prof) {
@@ -1187,36 +1188,40 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
 }
 
 // the instantiation is chosen by the rank layout of the call: 0 (float64 scan), 1, 2 or 4 packed words per row
-template <int D, bool BINS, bool PRUNE, bool SEL = false>
+template <int D, bool BINS, bool PRUNE, bool SEL = false, bool AA = false>
 static acsfit_status launch_pipeline_v(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
     switch (pp.rk.nw) {
-    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL>(ctx, pp, stages, st, resident);
-    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL>(ctx, pp, stages, st, resident);
-    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL>(ctx, pp, stages, st, resident);
-    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL>(ctx, pp, stages, st, resident);
+    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL, AA>(ctx, pp, stages, st, resident);
+    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL, AA>(ctx, pp, stages, st, resident);
+    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL, AA>(ctx, pp, stages, st, resident);
+    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL, AA>(ctx, pp, stages, st, resident);
     default: return fail(ctx, ACSFIT_E_INVALID, "rank layout with %d words", pp.rk.nw);
     }
 }
 
-// node pass with node selectors (pp.node_match != nullptr): the same pruning rule as below, barrier form only
-template <int D>
+// node pass with node selectors (pp.node_match != nullptr), AA: and anti-affinity masks: the same pruning rule as
+// below, barrier form only
+template <int D, bool AA = false>
 static acsfit_status launch_pipeline_sel(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
     int prune = ctx->prune;
     if (prune < 0) {
         int resident = 0;
-        TRY((launch_pipeline_v<D, false, false, true>(ctx, pp, stages, st, &resident)));
+        TRY((launch_pipeline_v<D, false, false, true, AA>(ctx, pp, stages, st, &resident)));
         prune = stages > resident;
     }
-    if (prune) return launch_pipeline_v<D, false, true, true>(ctx, pp, stages, st, nullptr);
-    return launch_pipeline_v<D, false, false, true>(ctx, pp, stages, st, nullptr);
+    if (prune) return launch_pipeline_v<D, false, true, true, AA>(ctx, pp, stages, st, nullptr);
+    return launch_pipeline_v<D, false, false, true, AA>(ctx, pp, stages, st, nullptr);
 }
 
 template <int D, bool BINS>
 static acsfit_status launch_pipeline_t(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
-    if (!BINS) {
+    if constexpr (BINS) {
+        if (pp.pod_carries) return launch_pipeline_v<D, true, false, false, true>(ctx, pp, stages, st, nullptr);
+    } else {
+        if (pp.pod_carries) return launch_pipeline_sel<D, true>(ctx, pp, stages, st);  // the entry point set node_match
         if (pp.node_match) return launch_pipeline_sel<D>(ctx, pp, stages, st);
         // Stage bounds + scan-list pruning (the PRUNE instantiation) pay when the pass is throughput-bound, i.e.
         // when there are more stages than the GPU holds at once (waves); a pass that fits is bound by its
@@ -1661,10 +1666,12 @@ static size_t first_fit_scratch(const acsfit_ctx *ctx, int64_t P, int64_t N)
 }
 
 // pod_class / node_match (device, both or neither): node selectors (the SEL form of the node pass; single GPU only)
+// aa (needs pod_class / node_match): anti-affinity masks (the SEL + AA form; single GPU only)
 static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const int32_t *pod_idx, int64_t P, int D,
                                     const double *cap_type, const int32_t *node_type, double *used, int64_t N,
                                     int32_t *out_placed, unsigned long long *out_decisions, cudaStream_t st,
-                                    const uint8_t *pod_class = nullptr, const unsigned long long *node_match = nullptr)
+                                    const uint8_t *pod_class = nullptr, const unsigned long long *node_match = nullptr,
+                                    const acsfit_anti_affinity *aa = nullptr)
 {
     if (ctx->world > 1)
         return cluster_first_fit(ctx, req, pod_idx, P, D, cap_type, node_type, used, N, out_placed, out_decisions, st);
@@ -1708,6 +1715,12 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
     pp.rk = ctx->rk;
     pp.pod_class = pod_class;
     pp.node_match = node_match;
+    if (aa) {
+        pp.pod_carries = reinterpret_cast<const unsigned long long *>(aa->pod_carries);
+        pp.pod_matches = reinterpret_cast<const unsigned long long *>(aa->pod_matches);
+        pp.node_carries = reinterpret_cast<unsigned long long *>(aa->node_carries);
+        pp.node_matches = reinterpret_cast<unsigned long long *>(aa->node_matches);
+    }
     unsigned long long *hits = nullptr;
     if (node_match) {
         hits = arena_take<unsigned long long>(ctx, 1);
@@ -1779,8 +1792,10 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                                   int64_t *out_new_size, int64_t *out_units_needed, int64_t *out_bins_opened,
                                   int32_t *out_acc_pool, int32_t *out_bin_of, int64_t *out_unaccounted,
                                   uint64_t *out_evals, cudaStream_t st, const FirstPassDone *pre = nullptr,
-                                  const uint8_t *pod_class = nullptr, const uint64_t *pool_match_host = nullptr)
+                                  const uint8_t *pod_class = nullptr, const uint64_t *pool_match_host = nullptr,
+                                  const acsfit_anti_affinity *aa = nullptr)
 {
+    // aa: anti-affinity masks of the pods (indexed like req rows); every bin pass runs the AA form, unchained
     // pod_class [dev] (indexed like req rows) + pool_match_host [host] T (visiting order): node selectors.  They only
     // change the pool gate: every bin of a pool carries the pool's labels, so the bin passes are the plain ones.
     for (int i = 0; i < T * D; ++i)
@@ -1914,6 +1929,10 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                 }
                 pp.watchdog_ns = (unsigned long long)ctx->watchdog_ms * 1000000ull;
                 pp.rk = ctx->rk;
+                if (aa) {
+                    pp.pod_carries = reinterpret_cast<const unsigned long long *>(aa->pod_carries);
+                    pp.pod_matches = reinterpret_cast<const unsigned long long *>(aa->pod_matches);
+                }
                 if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
                 ctx->rec_pool = t;
                 TRY(launch_pipeline<true>(ctx, D, pp, plan.stages, st));
@@ -2730,6 +2749,98 @@ extern "C" acsfit_status acsfit_scale_up_sel(acsfit_ctx *ctx, const double *req,
     return scale_up_impl(ctx, req, P, D, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, T,
                          over_provision, cap_type, node_type, used_inout, N, out_feasible, out_placed, out_new_size,
                          out_units_needed, out_bins_opened, out_acc_pool, out_counters, st, sel);
+}
+
+// ---------------------------------------------------------------------------------------------
+// required pod anti-affinity (include/acsfit.h, acsfit_anti_affinity): the *_aa entry points
+// ---------------------------------------------------------------------------------------------
+static acsfit_status check_aa_host(acsfit_ctx *ctx, const acsfit_anti_affinity *aa, int64_t rows, int64_t N,
+                                   const char *what)
+{
+    if (!aa) return fail(ctx, ACSFIT_E_INVALID, "%s: anti-affinity masks missing", what);
+    if (ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: pod anti-affinity is not supported in cluster mode", what);
+    if ((rows > 0 && (!aa->pod_carries || !aa->pod_matches)) || (N > 0 && (!aa->node_carries || !aa->node_matches)))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: anti-affinity field missing", what);
+    return ACSFIT_OK;
+}
+
+extern "C" acsfit_status acsfit_first_fit_nodes_aa(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                   const int32_t *node_type, double *used_inout, int64_t N,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   int32_t *out_placed, uint64_t *out_decisions,
+                                                   acsfit_stream_t stream)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
+        (P > 0 && (!req || !out_placed)) || (N > 0 && (!cap_type || !node_type || !used_inout)))
+        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_aa: bad arguments");
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_aa: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
+    TRY(check_req_aligned(ctx, req, "first_fit_nodes_aa"));
+    TRY(check_aa_host(ctx, aa, req_rows, N, "first_fit_nodes_aa"));
+    if (sel) TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, "first_fit_nodes_aa"));
+    reset_stats(ctx);
+    // without selectors: class 0 for every row and all-ones node masks, from the arena
+    const size_t trivial = sel ? 0 : align_up((size_t)req_rows, 256) + sizeof(uint64_t) * (size_t)N + 512;
+    TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + trivial + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_domain(ctx, req, req_rows * D, flag, st, "req"));
+    const uint8_t *pod_class;
+    const unsigned long long *node_match;
+    if (sel) {
+        TRY(check_classes(ctx, sel->pod_class, req_rows, sel->classes, flag, st, "first_fit_nodes_aa", sel->node_match, N));
+        pod_class = sel->pod_class;
+        node_match = reinterpret_cast<const unsigned long long *>(sel->node_match);
+    } else {
+        TAKE(cls0, uint8_t, req_rows);
+        TAKE(all, unsigned long long, N);
+        if (req_rows > 0) CUDA_TRY(cudaMemsetAsync(cls0, 0, (size_t)req_rows, st));
+        if (N > 0) CUDA_TRY(cudaMemsetAsync(all, 0xFF, sizeof(unsigned long long) * (size_t)N, st));
+        pod_class = cls0;
+        node_match = all;
+    }
+    if (P > 0 && N > 0) TRY(build_ranks(ctx, req, req_rows, D, st));
+    return first_fit_impl(ctx, req, pod_idx, P, D, cap_type, node_type, used_inout, N, out_placed,
+                          reinterpret_cast<unsigned long long *>(out_decisions), st, pod_class, node_match, aa);
+}
+
+extern "C" acsfit_status acsfit_fulfill_pending_aa(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                   int64_t num_listed, int D, const double *unit,
+                                                   const int32_t *pool_actual, const int32_t *pool_max,
+                                                   const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   int64_t *out_new_size, int64_t *out_units_needed,
+                                                   int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                                   int32_t *out_bin_of, int64_t *out_unaccounted,
+                                                   uint64_t *out_evals, acsfit_stream_t stream)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
+        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
+        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
+                   !out_bins_opened)) ||
+        !out_unaccounted)
+        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_aa: bad arguments");
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_aa: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
+    TRY(check_req_aligned(ctx, req, "fulfill_pending_aa"));
+    TRY(check_aa_host(ctx, aa, Pp, 0, "fulfill_pending_aa"));
+    if (sel) TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, "fulfill_pending_aa"));
+    reset_stats(ctx);
+    TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_domain(ctx, req, Pp * D, flag, st, "req"));
+    if (sel) TRY(check_classes(ctx, sel->pod_class, Pp, sel->classes, flag, st, "fulfill_pending_aa"));
+    TRY(build_ranks(ctx, req, Pp, D, st));
+    return fulfill_impl(ctx, req, nullptr, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                        over_provision, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
+                        out_unaccounted, out_evals, st, nullptr, sel ? sel->pod_class : nullptr,
+                        sel ? sel->pool_match_ordered : nullptr, aa);
 }
 
 // ---------------------------------------------------------------------------------------------

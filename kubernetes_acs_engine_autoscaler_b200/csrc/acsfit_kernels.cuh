@@ -132,6 +132,13 @@ struct PipelineParams {
     const uint8_t *pod_class;               // [req rows] selector class of each request row
     const unsigned long long *node_match;   // [N] classes each node matches
     unsigned long long *sel_hits;           // optional: += the scan's hit entries of every tile of every stage
+    // required pod anti-affinity (AA instantiations only; appended): bit k = term k.  A pod may take a node (bin) only
+    // when (pod_carries & node_matches) | (pod_matches & node_carries) == 0; the taker ORs the pod's masks into the
+    // node's.  Node passes read and write node_carries / node_matches; bins start at 0 and are not written back.
+    const unsigned long long *pod_carries;  // [req rows] terms the pod has
+    const unsigned long long *pod_matches;  // [req rows] terms that select the pod
+    unsigned long long *node_carries;       // [N] in/out (node pass)
+    unsigned long long *node_matches;       // [N] in/out (node pass)
 };
 
 __device__ __forceinline__ int ld_acquire(const int *p)
@@ -174,6 +181,12 @@ __device__ __forceinline__ void note_take(unsigned smem_addr, unsigned v, unsign
     asm volatile("{ .reg .pred p; setp.eq.u32 p, %2, 0; @p st.shared.u8 [%0], %1; }" ::"r"(smem_addr), "r"(v), "r"(loses) : "memory");
 }
 
+// m <- m | v when `loses` == 0 (AA: the taker's node masks gain the entry's bits, predicated like state_take)
+__device__ __forceinline__ void mask_take(unsigned long long &m, unsigned long long v, unsigned loses)
+{
+    asm("{ .reg .pred p; setp.eq.u32 p, %2, 0; @p or.b64 %0, %0, %1; }" : "+l"(m) : "l"(v), "r"(loses));
+}
+
 // S <- S -/+ r when `loses` == 0, as ONE predicated instruction in place (the compiler's own if-conversion computes
 // into a temporary and adds a predicated move per register half - one more dependent step on the placement chain).
 template <bool BINS>
@@ -200,7 +213,7 @@ __device__ __forceinline__ void load_row(double (&r)[D], const double *src)
 // dynamic shared memory layout (doubles first for alignment).
 // nodes mode keeps three [D][Tn] arrays: scan thresholds, used (the mutable state) and capacity;
 // bins mode keeps one: the remaining capacity IS the threshold (finite values, Lemma B).
-template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false>
+template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false, bool AA = false>
 struct PipelineSmem {
     static constexpr int NW = NT / 32;  // warps per stage CTA == resolver warps
     static __host__ __device__ size_t bytes(int Tn)
@@ -211,7 +224,8 @@ struct PipelineSmem {
                                      (NW - 1) * (kTile + 1) /*warp queues*/ + 1 /*pad*/)
                + sizeof(unsigned short) * kTile /*slot_of*/ + (size_t)NW * 32 /*accepted node per dense entry*/
                + sizeof(unsigned) * ((size_t)RW * Tn /*packed node words*/ + (size_t)RW * kTile /*packed pod words*/ + 4 /*alignment*/)
-               + (SEL ? sizeof(unsigned long long) * (size_t)Tn /*node masks*/ + kTile /*pod classes*/ + (size_t)NW * 36 /*batch classes*/ : 0);
+               + (SEL ? sizeof(unsigned long long) * (size_t)Tn /*node masks*/ + kTile /*pod classes*/ + (size_t)NW * 36 /*batch classes*/ : 0)
+               + (AA ? sizeof(unsigned long long) * 2 * ((size_t)Tn /*node carries / matches*/ + kTile /*pod masks*/ + (size_t)NW * 36 /*batch masks*/) : 0);
     }
 };
 
@@ -250,11 +264,19 @@ __device__ __forceinline__ unsigned wait_entry(const volatile unsigned *slot, in
 // superset filter of "fits AND matches"; the per-warp and per-stage bounds stay resource-only (see the PRUNE test in
 // the tile loader).  Bin passes need no SEL form: every bin of a pool carries the pool's labels, so the host gates the
 // pods by match before a bin pass and the "untouched bin takes every eligible pod" shortcut stays exact.
-template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false>
+//
+// AA (node passes with SEL, and bin passes): required pod anti-affinity.  Whether pod p may take node n depends on the
+// pods that reached n earlier in the pass, so it is not a static class: each node (bin) keeps two u64 term masks that
+// the taker ORs the entry's masks into, and the resolver ANDs "not blocked" into its vote.  A node's masks only gain
+// bits, so a pod blocked under older state is blocked now too: the resource-only (plus class) scan, the stale
+// thresholds, the bounds, pruning and the untouched-bin shortcut (a new bin has both masks 0 and blocks nobody) all
+// stay exact.  AA runs the barrier form only.
+template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false, bool AA = false>
 __global__ void __launch_bounds__(NT, D <= 4 ? 2 : 1)
 firstfit_pipeline_kernel(const PipelineParams p)
 {
     static_assert(!(SEL && BINS), "selectors apply to node passes only");
+    static_assert(!AA || BINS || SEL, "the anti-affinity node pass builds on the selector form");
     constexpr int K = nodes_per_thread(D, RW);  // RW: 32-bit words of a packed-rank row, 0 = float64 scan
     constexpr int NW = NT / 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -287,6 +309,14 @@ firstfit_pipeline_kernel(const PipelineParams p)
     unsigned long long *nm_s = reinterpret_cast<unsigned long long *>(rw_s + (size_t)RW * kTile);  // [Tn]
     unsigned char *cls_s = reinterpret_cast<unsigned char *>(nm_s + Tn);                           // [kTile]
     unsigned char *bcls_s = cls_s + kTile;                                                         // [NW][36]
+    // AA: carries / matches of the stage's nodes, of the tile's compacted pods and of each resolver batch (8-byte
+    // aligned: the SEL arrays above take a multiple of 8 bytes)
+    unsigned long long *nc_s = SEL ? reinterpret_cast<unsigned long long *>(bcls_s + NW * 36) : nm_s;  // [Tn]
+    unsigned long long *nx_s = nc_s + Tn;                                                               // [Tn]
+    unsigned long long *pc_s = nx_s + Tn;                                                               // [kTile]
+    unsigned long long *px_s = pc_s + kTile;                                                            // [kTile]
+    unsigned long long *bc_s = px_s + kTile;                                                            // [NW][36]
+    unsigned long long *bx_s = bc_s + NW * 36;                                                          // [NW][36]
 
     const int tid = threadIdx.x;
     const int lane = tid & 31;
@@ -343,6 +373,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
         for (int i = tid; i < Tn * RW; i += NT) tw_s[i] = 0;
     if constexpr (SEL)  // padding nodes match nothing (they never fit either)
         for (int n = tid; n < Tn; n += NT) nm_s[n] = n < n_valid ? __ldg(p.node_match + stage_lo + n) : 0ull;
+    if constexpr (AA)  // bins (and padding nodes) start empty
+        for (int n = tid; n < Tn; n += NT) {
+            nc_s[n] = !BINS && n < n_valid ? p.node_carries[stage_lo + n] : 0ull;
+            nx_s[n] = !BINS && n < n_valid ? p.node_matches[stage_lo + n] : 0ull;
+        }
     __syncthreads();
     // (n, d) -> field t' of the node's packed threshold row; callers zero the row first
     auto pack_field = [&](int i) {
@@ -409,6 +444,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
     double pre[D];
     unsigned prew[RW > 0 ? RW : 1];
     unsigned pre_cls = 0;  // SEL: the entry's selector class
+    unsigned long long pre_c = 0ull, pre_x = 0ull;  // AA: the entry's carries / matches
     auto prefetch_row = [&](int tile) {
         const int64_t j = (int64_t)(p.tile_lo + tile) * kTile + tid;
         if (tid < kTile && tile < p.num_tiles && j < p.M) {
@@ -426,6 +462,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 for (int w = 0; w < RW; ++w) prew[w] = __ldg(p.rk.packed + (size_t)row * RW + w);
             }
             if constexpr (SEL) pre_cls = __ldg(p.pod_class + row);
+            if constexpr (AA) {
+                pre_c = __ldg(p.pod_carries + row);
+                pre_x = __ldg(p.pod_matches + row);
+            }
         }
     };
     prefetch_row(0);
@@ -541,6 +581,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 for (int w = 0; w < RW; ++w) rw_s[pos * RW + w] = prew[w];
             }
             if constexpr (SEL) cls_s[pos] = (unsigned char)pre_cls;
+            if constexpr (AA) {
+                pc_s[pos] = pre_c;
+                px_s[pos] = pre_x;
+            }
         }
         prefetch_row(tile + 1);
         __syncthreads();
@@ -754,6 +798,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 unsigned touched_tile = 0u;  // nodes / bins of this warp that took a pod in this tile
                 unsigned long long my_nm = 0ull;  // SEL: the classes this lane's node matches
                 if constexpr (SEL) my_nm = n < Tn ? nm_s[n] : 0ull;
+                unsigned long long my_nc = 0ull, my_nx = 0ull;  // AA: this lane's node's carries / matches
+                if constexpr (AA) {
+                    my_nc = n < Tn ? nc_s[n] : 0ull;
+                    my_nx = n < Tn ? nx_s[n] : 0ull;
+                }
 
                 unsigned my_takes = 0;  // pods this lane's node / bin took in this tile
                 const volatile unsigned *in_q = warp == first_w ? hitlist : queue + (size_t)(warp - 1) * (kTile + 1);
@@ -831,11 +880,16 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     }
                     const int my_rank = __popc(possmask & ((1u << lane) - 1u));
                     unsigned char *bcls = bcls_s + warp * 36;  // SEL: class of each dense entry (+4 padding entries)
+                    unsigned long long *bc = bc_s + warp * 36, *bx = bx_s + warp * 36;  // AA: masks of each dense entry
                     if (poss) {
 #pragma unroll
                         for (int d = 0; d < D; d += 2)
                             *reinterpret_cast<double2 *>(brow + (size_t)my_rank * D + d) = make_double2(own[d], own[d + 1]);
                         if constexpr (SEL) bcls[my_rank] = cls_s[q_l];
+                        if constexpr (AA) {
+                            bc[my_rank] = pc_s[q_l];
+                            bx[my_rank] = px_s[q_l];
+                        }
                     }
                     fnd[lane] = 0xFF;  // "nobody took dense entry `lane`" until a taker says otherwise
                     const unsigned fnd_sa = (unsigned)__cvta_generic_to_shared(const_cast<unsigned char *>(fnd));
@@ -845,6 +899,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
 #pragma unroll
                         for (int d = 1; d < D; ++d) pad[d] = 0.0;
                         if constexpr (SEL) bcls[n_poss + lane] = 0;
+                        if constexpr (AA) {
+                            bc[n_poss + lane] = 0ull;
+                            bx[n_poss + lane] = 0ull;
+                        }
                     }
                     __syncwarp();
                     double r[D];
@@ -853,6 +911,13 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     // ahead, beside the row load, and is ready before the add-compare-vote chain needs it.
                     bool mt = true;
                     if constexpr (SEL) mt = ((my_nm >> bcls[0]) & 1ull) != 0ull;
+                    // AA: the entry's masks, loaded one entry ahead; the block test itself needs the node masks the
+                    // previous vote left, so it is evaluated beside the resource test
+                    unsigned long long ec = 0ull, ex = 0ull;
+                    if constexpr (AA) {
+                        ec = bc[0];
+                        ex = bx[0];
+                    }
                     const long long t_l0 = tracing ? clock64() : 0;
                     if (tracing) n_iter += (unsigned)n_poss;
                     // The placement chain.  Entry k's test needs the state left by entry k-1, which is only known once the
@@ -884,8 +949,14 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         load_row<D>(r_next, brow + (size_t)(k + 1) * D);
                         bool mt_next = true;
                         if constexpr (SEL) mt_next = ((my_nm >> bcls[k + 1]) & 1ull) != 0ull;
+                        unsigned long long ec_next = 0ull, ex_next = 0ull;
+                        if constexpr (AA) {
+                            ec_next = bc[k + 1];
+                            ex_next = bx[k + 1];
+                        }
                         bool ok = fits(S, r);
                         if constexpr (SEL) ok = ok & mt;
+                        if constexpr (AA) ok = ok & (((ec & my_nx) | (ex & my_nc)) == 0ull);
                         // the vote-to-vote path: ballot -> "no fitting lane before me" -> predicated update of S -> next
                         // test.  No branch on it (at the frontier nearly every entry is taken) and no mask arithmetic
                         // beyond one and + compare.
@@ -893,11 +964,19 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         const unsigned loses = (m & le) ^ me;  // 0 <=> this is the first fitting node of the warp
 #pragma unroll
                         for (int d = 0; d < D; ++d) state_take<BINS>(S[d], r[d], loses);  // scaler.py:140 / kube.py:171
+                        if constexpr (AA) {
+                            mask_take(my_nc, ec, loses);
+                            mask_take(my_nx, ex, loses);
+                        }
                         note_take(fnd_sa + (unsigned)k, (unsigned)lane, loses);  // off the chain: who took entry k
                         my_takes += loses ? 0u : 1u;
 #pragma unroll
                         for (int d = 0; d < D; ++d) r[d] = r_next[d];
                         if constexpr (SEL) mt = mt_next;
+                        if constexpr (AA) {
+                            ec = ec_next;
+                            ex = ex_next;
+                        }
                     }
                     __syncwarp();
                     {
@@ -946,6 +1025,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     if (n < Tn) {
 #pragma unroll
                         for (int d = 0; d < D; ++d) state_s[(size_t)d * Tn + n] = S[d];
+                        if constexpr (AA) {
+                            nc_s[n] = my_nc;
+                            nx_s[n] = my_nx;
+                        }
                     }
                     if (lane == 0) {
                         if (BINS) opened[warp] = touched_or_open;
@@ -1033,6 +1116,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
             const int n = i / D, d = i - n * D;
             if (n < n_valid) p.used[(size_t)(stage_lo + n) * D + d] = state_s[(size_t)d * Tn + n];
         }
+        if constexpr (AA)
+            for (int n = tid; n < n_valid; n += NT) {
+                p.node_carries[stage_lo + n] = nc_s[n];
+                p.node_matches[stage_lo + n] = nx_s[n];
+            }
     }
     if (BINS && lane == 0 && my_evals) atomicAdd(p.evals, my_evals);  // every warp credits its own placements
     if (tid == 0) {

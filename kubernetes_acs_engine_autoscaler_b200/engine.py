@@ -418,6 +418,64 @@ class Engine(object):
                     "num_unaccounted": int(counters[2]), "decisions": int(counters[3])})
         return res
 
+    # ------------------------------------------------------------------ pod anti-affinity (include/acsfit.h)
+    @staticmethod
+    def _anti_affinity(pod_carries, pod_matches, node_carries=None, node_matches=None):
+        """(struct acsfit_anti_affinity, the tensors it points to -- keep them alive over the call); device tensors."""
+        keep = [pod_carries, pod_matches, node_carries, node_matches]
+        aa = _native.AntiAffinity(*[None if a is None else _ptr(a).value for a in keep])
+        return aa, keep
+
+    def first_fit_nodes_aa(self, req, pod_idx, cap_type, node_type, used, pod_carries, pod_matches, node_carries,
+                           node_matches, pod_class=None, node_match=None, classes=1):
+        """first_fit_nodes with required pod anti-affinity: pod_carries / pod_matches uint64 [req rows] device (stored
+        as int64), node_carries / node_matches uint64 [N] device, updated in place like `used`.  pod_class /
+        node_match (both or neither): node selectors as in first_fit_nodes_sel."""
+        rows, D = req.shape
+        P = rows if pod_idx is None else pod_idx.shape[0]
+        N = used.shape[0]
+        placed = self.empty((P,), torch.int32)
+        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
+        sel, keep_s = (None, None) if pod_class is None else \
+            self._selectors(classes, pod_class=pod_class, node_match=node_match)
+        aa, keep_a = self._anti_affinity(pod_carries, pod_matches, node_carries, node_matches)
+        self._check(self._lib.acsfit_first_fit_nodes_aa(
+            self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
+            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
+            ctypes.cast(ctypes.byref(aa), ctypes.c_void_p), _ptr(placed), _ptr(decisions), self._stream()))
+        return placed, decisions
+
+    def fulfill_pending_aa(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision,
+                           pod_carries, pod_matches, pod_class=None, pool_match=None, classes=1):
+        """fulfill_pending with required pod anti-affinity in the bins: pod_carries / pod_matches uint64 [Pp] device
+        (stored as int64).  pod_class / pool_match (both or neither): node selectors as in fulfill_pending_sel."""
+        Pp, D = req.shape
+        unit = _np(unit, np.float64).reshape(-1, D)
+        T = unit.shape[0]
+        pool_actual = _np(pool_actual, np.int32)
+        pool_max = _np(pool_max, np.int32)
+        pool_ignored = _np(pool_ignored, np.uint8)
+        new_size = np.zeros(T, dtype=np.int64)
+        units_needed = np.zeros(T, dtype=np.int64)
+        bins_opened = np.zeros(T, dtype=np.int64)
+        acc_pool = self.empty((Pp,), torch.int32)
+        bin_of = self.empty((Pp,), torch.int32)
+        unacc = ctypes.c_int64(0)
+        evals = ctypes.c_uint64(0)
+        sel, keep_s = (None, None) if pod_class is None else \
+            self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
+        aa, keep_a = self._anti_affinity(pod_carries, pod_matches)
+        self._check(self._lib.acsfit_fulfill_pending_aa(
+            self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
+            _ptr(pool_ignored), T, int(over_provision),
+            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
+            ctypes.cast(ctypes.byref(aa), ctypes.c_void_p), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened),
+            _ptr(acc_pool), _ptr(bin_of), ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p),
+            ctypes.cast(ctypes.byref(evals), ctypes.c_void_p), self._stream()))
+        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
+                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
+                "evals": int(evals.value)}
+
     # ------------------------------------------------------------------ host-buffer entry points
     def scale_up_host(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,
                       cap_type, node_type, used, out=None):

@@ -82,6 +82,95 @@ def tolerates_all(tolerations, taints):
     return all(tolerates(tolerations, t) for t in taints)
 
 
+# required pod anti-affinity: only terms with this topology key are honoured (one node = one topology domain)
+HOSTNAME_TOPOLOGY_KEY = 'kubernetes.io/hostname'
+SELECTOR_OPERATORS = ('In', 'NotIn', 'Exists', 'DoesNotExist')
+
+
+def _str_list(value, what, owner):
+    if not isinstance(value, list) or not all(isinstance(v, str) for v in value):
+        raise ValueError("malformed %s of %s: expected a list of strings, got %r" % (what, owner, value))
+    return value
+
+
+def _mapping(value, what, owner):
+    if not isinstance(value, Mapping):
+        raise ValueError("malformed %s of %s: expected a mapping, got %r" % (what, owner, value))
+    return value
+
+
+def label_selector(selector, owner, what='labelSelector'):
+    """the canonical, hashable form of a metav1.LabelSelector: (sorted matchLabels items, sorted (key, operator, sorted
+    values) requirements).  Two selectors with equal forms select the same pods.  ValueError naming the owner when the
+    selector is malformed (unknown operator, values with Exists / DoesNotExist, no values with In / NotIn)."""
+    _mapping(selector, what, owner)
+    labels = selector.get('matchLabels') or {}
+    _mapping(labels, what + '.matchLabels', owner)
+    if not all(isinstance(k, str) and isinstance(v, str) for k, v in labels.items()):
+        raise ValueError("malformed %s.matchLabels of %s: %r" % (what, owner, labels))
+    reqs = []
+    for e in _entries(selector.get('matchExpressions'), what + '.matchExpressions', owner):
+        key, op = e.get('key'), e.get('operator')
+        values = e.get('values')
+        values = [] if values is None else _str_list(values, what + '.matchExpressions.values', owner)
+        if not isinstance(key, str) or op not in SELECTOR_OPERATORS or \
+                (op in ('In', 'NotIn')) != bool(values):
+            raise ValueError("malformed %s.matchExpressions entry of %s: %r" % (what, owner, e))
+        reqs.append((key, op, tuple(sorted(set(values)))))
+    return tuple(sorted(labels.items())), tuple(sorted(set(reqs)))
+
+
+def selector_matches(selector, labels):
+    """the canonical selector (label_selector) selects a pod with these labels (an empty selector selects every pod;
+    NotIn and DoesNotExist hold when the key is absent)"""
+    items, reqs = selector
+    for key, value in items:
+        if labels.get(key) != value:
+            return False
+    for key, op, values in reqs:
+        have = labels.get(key)
+        if op == 'In':
+            ok = have is not None and have in values
+        elif op == 'NotIn':
+            ok = have is None or have not in values
+        elif op == 'Exists':
+            ok = have is not None
+        else:
+            ok = have is None
+        if not ok:
+            return False
+    return True
+
+
+def anti_affinity_terms(affinity, namespace, owner):
+    """the required pod anti-affinity terms of spec.affinity that this project honours, as (namespaces, selector)
+    pairs: frozenset of namespaces (empty `namespaces` = the carrying pod's own), canonical label_selector.  Only terms
+    with topologyKey kubernetes.io/hostname count; a term with an absent or null labelSelector selects no pod and a
+    term with a namespaceSelector is not honoured, so both are left out.  ValueError naming the owner when a field
+    is malformed."""
+    if affinity is None:
+        return ()
+    _mapping(affinity, 'spec.affinity', owner)
+    anti = affinity.get('podAntiAffinity')
+    if anti is None:
+        return ()
+    _mapping(anti, 'spec.affinity.podAntiAffinity', owner)
+    what = 'spec.affinity.podAntiAffinity.requiredDuringSchedulingIgnoredDuringExecution'
+    terms = []
+    for t in _entries(anti.get('requiredDuringSchedulingIgnoredDuringExecution'), what, owner):
+        topology = t.get('topologyKey')
+        if not isinstance(topology, str):
+            raise ValueError("malformed %s entry of %s: topologyKey %r" % (what, owner, topology))
+        namespaces = t.get('namespaces')
+        namespaces = [] if namespaces is None else _str_list(namespaces, what + '.namespaces', owner)
+        selector = t.get('labelSelector')
+        selector = None if selector is None else label_selector(selector, owner, what + '.labelSelector')
+        if topology != HOSTNAME_TOPOLOGY_KEY or selector is None or t.get('namespaceSelector') is not None:
+            continue
+        terms.append((frozenset(namespaces) if namespaces else frozenset((namespace,)), selector))
+    return tuple(dict.fromkeys(terms))
+
+
 class KubePodStatus(object):
     RUNNING = 'Running'
     PENDING = 'Pending'
@@ -223,6 +312,11 @@ class KubePod(object):
         """spec.tolerations ([] when absent); read on use, so pods built attribute by attribute (make_pods) have it too.
         ValueError when it is not a list of mappings."""
         return _entries(self.original.obj['spec'].get('tolerations'), 'spec.tolerations', 'pod %s' % self)
+
+    @property
+    def anti_affinity_terms(self):
+        """the honoured required pod anti-affinity terms (kube.anti_affinity_terms); read on use, like tolerations."""
+        return anti_affinity_terms(self.original.obj['spec'].get('affinity'), self.namespace, 'pod %s' % self)
 
     def is_mirrored(self):
         daemonset = self._created_by().get('reference', {}).get('kind') == 'DaemonSet'

@@ -67,6 +67,8 @@ class Scaler(object):
         # with node selectors: a pod matches a node or pool only when it also tolerates its blocking taints
         # (Cluster(node_taints=...))
         self.node_taints = False
+        # required pod anti-affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_anti_affinity=...))
+        self.pod_anti_affinity = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -98,8 +100,9 @@ class Scaler(object):
         classes = None
         if self.node_selectors:
             classes = snapshot.selector_classes(unique, [], ordered_pools, taints=self.node_taints)
+        anti_affinity = snapshot.anti_affinity(unique) if self.pod_anti_affinity else None
         res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision,
-                               classes=classes)
+                               classes=classes, anti_affinity=anti_affinity)
 
         new_pool_sizes, current_pool_sizes = {}, {}
         unaccounted = len(pods)

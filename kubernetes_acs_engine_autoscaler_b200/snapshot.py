@@ -9,6 +9,8 @@ Layout: resource dims = sorted union of keys over every vector involved; a missi
 (bit-exact with KubeResource's own missing-key rule, kube.py:204-206,:210-212); the column count
 is padded with zero columns to 2/4/8/16 for the first-fit kernels.
 """
+import itertools
+
 import numpy as np
 import torch
 
@@ -305,6 +307,149 @@ def pending_match(pods, nodes, taints=False):
 
 
 # ------------------------------------------------------------------------------------------------
+# required pod anti-affinity: term masks (include/acsfit.h, acsfit_anti_affinity)
+# ------------------------------------------------------------------------------------------------
+MAX_AA_TERMS = 64
+
+
+class AntiAffinity(object):
+    """pod_carries / pod_matches uint64[P] (the terms each pod has / the terms that select it), node_carries /
+    node_matches uint64[N] (the OR of both over the pods already on each node) and the number of terms.  Bit k = term k
+    of `terms`, a list of (namespaces, canonical selector)."""
+
+    def __init__(self, pod_carries, pod_matches, node_carries, node_matches, terms):
+        self.pod_carries = pod_carries
+        self.pod_matches = pod_matches
+        self.node_carries = node_carries
+        self.node_matches = node_matches
+        self.terms = terms
+
+    @property
+    def trivial(self):
+        """no term can block a pod of this call: the plain entry points give the same result"""
+        return not self.terms
+
+
+def _pod_projection(pods, keys):
+    """(group[len(pods)], proj[G, 1 + len(keys)], code_of): the pods grouped by (namespace, the values of the label keys
+    the terms read), as _Projection groups nodes.  Column 0 numbers the namespace, column 1 + k the value of keys[k]
+    (None when absent); code_of[c] maps a value of column c to its number."""
+    columns = [[p.namespace for p in pods]]
+    labels = [p.labels for p in pods] if keys else []
+    for key in keys:
+        columns.append([l.get(key) for l in labels])
+    codes, code_of = [], []
+    for values in columns:
+        code = {v: i for i, v in enumerate(dict.fromkeys(values))}
+        code_of.append(code)
+        codes.append(np.fromiter(map(code.__getitem__, values), dtype=np.int64, count=len(values)))
+    if not len(pods):
+        return np.zeros(0, np.int64), np.zeros((0, len(columns)), np.int64), code_of
+    stacked = np.stack(codes, axis=1)
+    proj, group = np.unique(stacked, axis=0, return_inverse=True)
+    return group.reshape(-1), proj, code_of
+
+
+def _term_selects(term, proj, code_of, column):
+    """bool[G]: the term (namespaces, canonical selector) selects the pods of each projection"""
+    namespaces, (items, reqs) = term
+    hit = np.isin(proj[:, 0], [code_of[0][ns] for ns in namespaces if ns in code_of[0]])
+
+    def codes(key, values):
+        return [code_of[column[key]][v] for v in values if v in code_of[column[key]]]
+    for key, value in items:
+        hit &= np.isin(proj[:, column[key]], codes(key, (value,)))
+    for key, op, values in reqs:
+        col = proj[:, column[key]]
+        if op == 'In':
+            hit &= np.isin(col, codes(key, values))
+        elif op == 'NotIn':
+            hit &= ~np.isin(col, codes(key, values))
+        elif op == 'Exists':
+            hit &= ~np.isin(col, codes(key, (None,)))
+        else:
+            hit &= np.isin(col, codes(key, (None,)))
+    return hit
+
+
+def anti_affinity(pods, nodes=(), running_pods=()):
+    """term masks of the pods to place (`pods`) and of the nodes (the pods of `running_pods` on them count, matched by
+    node name as the occupancy count matches them).  A term (KubePod.anti_affinity_terms) is kept only when it can
+    block a pod to place: a pod to place carries it and it selects some other pod, or it selects a pod to place and some
+    other pod carries it.  (A lone replica of a self-anti-affine deployment blocks nothing, so its term is dropped.)  The
+    bin pass calls this with the pending pods alone: only they meet in new bins.  Kept terms are numbered in
+    first-occurrence order; ValueError above 64.  Each term is evaluated once per distinct (namespace, label values it
+    reads) projection of the pods, vectorised, not once per pod; nothing of size pods x terms is built."""
+    pods, nodes = list(pods), list(nodes)
+    row_ptr, run_idx = running_csr(nodes, running_pods) if nodes and running_pods else (None, np.zeros(0, np.int32))
+    running = list(running_pods)
+    on_nodes = np.unique(run_idx)
+    everyone = pods + [running[j] for j in on_nodes.tolist()]
+    P = len(pods)
+    term_id, terms = {}, []
+    carried = []  # per pod of `everyone`: its term numbers (before dropping)
+    for p in everyone:
+        ids = []
+        for t in p.anti_affinity_terms:
+            k = term_id.get(t)
+            if k is None:
+                k = term_id[t] = len(terms)
+                terms.append(t)
+            ids.append(k)
+        carried.append(ids)
+    if not terms:
+        return AntiAffinity(np.zeros(P, np.uint64), np.zeros(P, np.uint64), np.zeros(len(nodes), np.uint64),
+                            np.zeros(len(nodes), np.uint64), [])
+    T = len(terms)
+    keys = sorted({key for _, (items, reqs) in terms for key, *_ in items + reqs})
+    group, proj, code_of = _pod_projection(everyone, keys)
+    column = {key: 1 + k for k, key in enumerate(keys)}
+    G = len(proj)
+    # (pod, term) pairs of the carried terms (anti_affinity_terms lists a term once per pod)
+    lens = np.fromiter(map(len, carried), dtype=np.int64, count=len(everyone))
+    pair_pod = np.repeat(np.arange(len(everyone), dtype=np.int64), lens)
+    pair_term = np.fromiter(itertools.chain.from_iterable(carried), dtype=np.int64, count=int(lens.sum()))
+    to_place = pair_pod < P
+    n_carry = np.bincount(pair_term, minlength=T)               # pods that carry the term
+    n_carry_p = np.bincount(pair_term[to_place], minlength=T)   # ... pods to place among them
+    per_group = np.bincount(group, minlength=G)
+    per_group_p = np.bincount(group[:P], minlength=G)
+    order = np.argsort(pair_term[to_place], kind="stable")
+    carrier_p, bounds = pair_pod[to_place][order], np.searchsorted(pair_term[to_place][order], np.arange(T + 1))
+    n_sel, n_sel_p, n_both_p = (np.zeros(T, np.int64) for _ in range(3))  # selected pods, to place, to place + carrier
+    for t in range(T):
+        hit = _term_selects(terms[t], proj, code_of, column)
+        n_sel[t], n_sel_p[t] = per_group[hit].sum(), per_group_p[hit].sum()
+        n_both_p[t] = hit[group[carrier_p[bounds[t]:bounds[t + 1]]]].sum()
+    # a pair of two different pods, one to place, where one carries the term and it selects the other: the only
+    # carrier-and-selected pod of each count being the same pod is the one way to have counts but no such pair
+    alone = n_both_p == 1
+    relevant = ((n_carry_p >= 1) & (n_sel >= 1) & ~((n_sel == 1) & (n_carry_p == 1) & alone)) | \
+        ((n_sel_p >= 1) & (n_carry >= 1) & ~((n_carry == 1) & (n_sel_p == 1) & alone))
+    keep = np.nonzero(relevant)[0]
+    if len(keep) > MAX_AA_TERMS:
+        raise ValueError("more than %d distinct pod anti-affinity terms are not supported" % MAX_AA_TERMS)
+    bit_of = np.full(T, -1, dtype=np.int64)
+    bit_of[keep] = np.arange(len(keep))
+    group_matches = np.zeros(G, dtype=np.uint64)
+    for k, t in enumerate(keep.tolist()):
+        group_matches[_term_selects(terms[t], proj, code_of, column)] |= np.uint64(1) << np.uint64(k)
+    matches = group_matches[group]
+    carries = np.zeros(len(everyone), dtype=np.uint64)
+    kept = bit_of[pair_term] >= 0
+    np.bitwise_or.at(carries, pair_pod[kept], np.uint64(1) << bit_of[pair_term[kept]].astype(np.uint64))
+    node_carries = np.zeros(len(nodes), dtype=np.uint64)
+    node_matches = np.zeros(len(nodes), dtype=np.uint64)
+    if len(run_idx):
+        # OR over the running pods of each node (a pod is in `everyone` at P + its rank in on_nodes)
+        at = P + np.searchsorted(on_nodes, run_idx)
+        node_of = np.repeat(np.arange(len(nodes), dtype=np.int64), np.diff(row_ptr))
+        np.bitwise_or.at(node_carries, node_of, carries[at])
+        np.bitwise_or.at(node_matches, node_of, matches[at])
+    return AntiAffinity(carries[:P], matches[:P], node_carries, node_matches, [terms[k] for k in keep.tolist()])
+
+
+# ------------------------------------------------------------------------------------------------
 # K0: feasibility (capacity.is_possible over the pools)
 # ------------------------------------------------------------------------------------------------
 def feasible_pods(pods, agent_pools, classes=None):
@@ -376,9 +521,11 @@ def count_running_pods(nodes, running_pods):
 # ------------------------------------------------------------------------------------------------
 # first fit over nodes (Cluster.get_pending_pods)
 # ------------------------------------------------------------------------------------------------
-def first_fit_nodes(pods, nodes, classes=None):
+def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None):
     """returns placed[len(pods)] (node index or -1) and mutates node.used_capacity like count_pod.  With `classes`
-    (selector_classes(pods, nodes, [])) a pod only takes a node that matches its nodeSelector."""
+    (selector_classes(pods, nodes, [])) a pod only takes a node that matches its nodeSelector.  With `anti_affinity`
+    (anti_affinity(pods, nodes, running_pods)) a pod only takes a node its required anti-affinity does not block; the
+    node masks are updated in place."""
     pods, nodes = list(pods), list(nodes)
     placed = np.full(len(pods), -1, dtype=np.int32)
     if not pods or not nodes:
@@ -392,7 +539,21 @@ def first_fit_nodes(pods, nodes, classes=None):
     req[bad] = 0.0
     eng = get_engine()
     d_used = eng.dev(used, torch.float64)
-    if classes is not None and not classes.trivial:
+    sel = classes is not None and not classes.trivial
+    if anti_affinity is not None and not anti_affinity.trivial:
+        aa = anti_affinity
+        d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
+        d_placed, _ = eng.first_fit_nodes_aa(eng.dev(req, torch.float64),
+                                             None if not bad.any() else eng.dev(ok_idx, torch.int32),
+                                             eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
+                                             eng.dev(aa.pod_carries.view(np.int64), torch.int64),
+                                             eng.dev(aa.pod_matches.view(np.int64), torch.int64), d_nc, d_nx,
+                                             *((eng.dev(classes.pod_class, torch.uint8),
+                                                eng.dev(classes.node_match.view(np.int64), torch.int64),
+                                                classes.classes) if sel else ()))
+        aa.node_carries[:] = d_nc.cpu().numpy().view(np.uint64)
+        aa.node_matches[:] = d_nx.cpu().numpy().view(np.uint64)
+    elif sel:
         d_placed, _ = eng.first_fit_nodes_sel(eng.dev(req, torch.float64),
                                               None if not bad.any() else eng.dev(ok_idx, torch.int32),
                                               eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
@@ -434,9 +595,11 @@ def single_can_fit(node, resources):
 # ------------------------------------------------------------------------------------------------
 # fulfill_pending (bins)
 # ------------------------------------------------------------------------------------------------
-def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_provision, classes=None):
+def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_provision, classes=None,
+            anti_affinity=None):
     """Scaler.fulfill_pending's packing + size arithmetic; pools already in visiting order.  With `classes`
-    (selector_classes(unique_pods, [], ordered_pools)) a pool only takes the pods whose nodeSelector it matches."""
+    (selector_classes(unique_pods, [], ordered_pools)) a pool only takes the pods whose nodeSelector it matches.  With
+    `anti_affinity` (anti_affinity(unique_pods)) a pod only takes a bin its required anti-affinity does not block."""
     from . import capacity
     units = [capacity.RESOURCE_SPEC[pool.instance_type] for pool in ordered_pools]
     dims = Dims([p.resources for p in unique_pods] + units)
@@ -448,7 +611,14 @@ def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_pro
     pools = (np.asarray([pool.actual_capacity for pool in ordered_pools], dtype=np.int32),
              np.asarray([min(pool.max_size, 2 ** 31 - 1) for pool in ordered_pools], dtype=np.int32),
              np.asarray([1 if pool.name in ignored_pool_names else 0 for pool in ordered_pools], dtype=np.uint8))
-    if classes is not None and not classes.trivial:
+    sel = classes is not None and not classes.trivial
+    if anti_affinity is not None and not anti_affinity.trivial:
+        res = eng.fulfill_pending_aa(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
+                                     eng.dev(anti_affinity.pod_carries.view(np.int64), torch.int64),
+                                     eng.dev(anti_affinity.pod_matches.view(np.int64), torch.int64),
+                                     *((eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
+                                       if sel else ()))
+    elif sel:
         res = eng.fulfill_pending_sel(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
                                       eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
     else:
