@@ -55,7 +55,7 @@ class Cluster(object):
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
-                 node_taints=None, pod_anti_affinity=None):
+                 node_taints=None, pod_anti_affinity=None, node_affinity=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -77,6 +77,14 @@ class Cluster(object):
         elif node_taints and not self.node_selectors:
             raise ValueError("node_taints=True needs node_selectors on")
         self.node_taints = bool(node_taints) and self.node_selectors
+        # with node selectors on, a pod matches a node or pool only when its required node affinity admits it too, so a
+        # pod pinned to a pool by affinity neither "fits" other pools' nodes nor holds them back (opt-in; None:
+        # $ACSFIT_NODE_AFFINITY)
+        if node_affinity is None:
+            node_affinity = os.environ.get('ACSFIT_NODE_AFFINITY', '0') not in ('', '0')
+        elif node_affinity and not self.node_selectors:
+            raise ValueError("node_affinity=True needs node_selectors on")
+        self.node_affinity = bool(node_affinity) and self.node_selectors
         # honour required pod anti-affinity with topologyKey kubernetes.io/hostname in first fit and bin packing, so that
         # replicas which avoid each other are not simulated onto one node (opt-in; None: $ACSFIT_POD_ANTI_AFFINITY).
         # Independent of node_selectors; with both on, the node pass uses both.
@@ -184,7 +192,7 @@ class Cluster(object):
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
             idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
             selector_node_states=self.selector_node_states, node_taints=self.node_taints,
-            pod_anti_affinity=self.pod_anti_affinity)
+            pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [
@@ -218,7 +226,7 @@ class Cluster(object):
         pods, nodes = list(pods), list(nodes)
         classes = None
         if self.node_selectors:
-            classes = snapshot.selector_classes(pods, nodes, [], taints=self.node_taints)
+            classes = snapshot.selector_classes(pods, nodes, [], taints=self.node_taints, affinity=self.node_affinity)
         anti_affinity = None
         if self.pod_anti_affinity:
             anti_affinity = snapshot.anti_affinity(pods, nodes, running_pods or [])
@@ -251,20 +259,31 @@ class Cluster(object):
         pending_unassigned_pods = [p for p in pods if p.status == KubePodStatus.PENDING and (not p.node_name)]
         classes = None
         if self.node_selectors:
-            classes = snapshot.selector_classes(pending_unassigned_pods, [], agent_pools, taints=self.node_taints)
+            classes = snapshot.selector_classes(pending_unassigned_pods, [], agent_pools, taints=self.node_taints,
+                                                affinity=self.node_affinity)
         feasible = snapshot.feasible_pods(pending_unassigned_pods, agent_pools, classes=classes)
         unmatched = set()  # rejected only because no pool that would fit matches the node selector
-        untolerated = set()  # some pool that would fit matches the selector, but each has a taint the pod does not tolerate
+        unaffine = set()  # some pool that would fit matches the selector, but none matches the required node affinity
+        untolerated = set()  # some pool that would fit matches selector and affinity, but each has an untolerated taint
         if classes is not None and not classes.trivial:
             rejected = [p for p, ok, c in zip(pending_unassigned_pods, feasible, classes.pod_class) if not ok and c]
             if rejected:
                 fits = snapshot.feasible_pods(rejected, agent_pools)
                 unmatched = {id(p) for p, ok in zip(rejected, fits) if ok}
-            if unmatched and self.node_taints:
+            if unmatched and (self.node_taints or self.node_affinity):
                 fitting = [p for p in rejected if id(p) in unmatched]
-                selected = snapshot.feasible_pods(fitting, agent_pools,
+                admitted = snapshot.feasible_pods(fitting, agent_pools,
                                                   classes=snapshot.selector_classes(fitting, [], agent_pools))
-                untolerated = {id(p) for p, ok in zip(fitting, selected) if ok}
+                selected = [p for p, a in zip(fitting, admitted) if a]
+                if self.node_affinity and self.node_taints:
+                    admitted = snapshot.feasible_pods(selected, agent_pools, classes=snapshot.selector_classes(
+                        selected, [], agent_pools, affinity=True))
+                    untolerated = {id(p) for p, a in zip(selected, admitted) if a}
+                    unaffine = {id(p) for p in selected} - untolerated
+                elif self.node_affinity:
+                    unaffine = {id(p) for p in selected}
+                else:
+                    untolerated = {id(p) for p in selected}
         pods_to_schedule = []
         warn = logger.isEnabledFor(logging.WARNING)  # (the message is formatted eagerly, as upstream: skip it when nobody listens)
         for pod, ok in zip(pending_unassigned_pods, feasible):
@@ -273,6 +292,9 @@ class Cluster(object):
             elif warn and id(pod) in untolerated:
                 logger.warning("Pending pod %s cannot fit: every agent pool that would fit it and matches its node "
                                "selector has a taint it does not tolerate. Scheduling skipped." % pod.name)
+            elif warn and id(pod) in unaffine:
+                logger.warning("Pending pod %s cannot fit: no agent pool that would fit it matches its required node "
+                               "affinity. Scheduling skipped." % pod.name)
             elif warn and id(pod) in unmatched:
                 logger.warning("Pending pod %s cannot fit: no agent pool matches its node selector %s. "
                                "Scheduling skipped." % (pod.name, pod.selectors))

@@ -22,12 +22,13 @@ ACT_NONE, ACT_CORDON_DRAIN, ACT_CORDON, ACT_UNCORDON, ACT_SCALE_IN = range(5)
 class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                  deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
-                 selector_node_states=False, node_taints=False, pod_anti_affinity=False):
+                 selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
         self.selector_node_states = selector_node_states
         self.node_taints = node_taints
+        self.node_affinity = node_affinity
         self.pod_anti_affinity = pod_anti_affinity
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template

@@ -10,6 +10,7 @@ import datetime
 import json
 import logging
 import os
+import re
 from collections.abc import Mapping
 
 from . import utils
@@ -171,6 +172,116 @@ def anti_affinity_terms(affinity, namespace, owner):
     return tuple(dict.fromkeys(terms))
 
 
+# required node affinity: the operators of a NodeSelectorRequirement, and the one field a matchFields entry may name
+NODE_SELECTOR_OPERATORS = ('In', 'NotIn', 'Exists', 'DoesNotExist', 'Gt', 'Lt')
+NODE_NAME_FIELD = 'metadata.name'
+_INT64 = re.compile(r'[+-]?[0-9]+')
+
+
+def parse_int64(text):
+    """Go's strconv.ParseInt(text, 10, 64): an optional sign, then ASCII digits, within int64; None otherwise (no
+    spaces or underscores, unlike int())"""
+    if type(text) is not str or not _INT64.fullmatch(text):
+        return None
+    value = int(text)
+    return value if -(1 << 63) <= value < (1 << 63) else None
+
+
+def _node_requirements(entries, what, owner, fields):
+    reqs = []
+    for e in _entries(entries, what, owner):
+        key, op = e.get('key'), e.get('operator')
+        values = e.get('values')
+        values = [] if values is None else _str_list(values, what + '.values', owner)
+        if fields:
+            ok = key == NODE_NAME_FIELD and op in ('In', 'NotIn') and len(values) == 1
+        elif op in ('In', 'NotIn'):
+            ok = bool(values)
+        elif op in ('Gt', 'Lt'):
+            ok = len(values) == 1 and parse_int64(values[0]) is not None
+            values = [parse_int64(values[0])] if ok else values
+        else:
+            ok = op in ('Exists', 'DoesNotExist') and not values
+        if not isinstance(key, str) or not ok:
+            raise ValueError("malformed %s entry of %s: %r" % (what, owner, e))
+        reqs.append((key, op, tuple(sorted(set(values)))))
+    return tuple(sorted(set(reqs)))
+
+
+def node_affinity_terms(affinity, owner):
+    """the canonical, hashable form of spec.affinity.nodeAffinity.requiredDuringSchedulingIgnoredDuringExecution: None
+    when there is no constraint (no affinity, no nodeAffinity, or a null required part; the preferred part is a scoring
+    preference and is ignored), else a sorted tuple of the nodeSelectorTerms that can match, each (sorted matchExpressions
+    requirements, sorted matchFields requirements) with a requirement (key, operator, sorted values); Gt / Lt values
+    are parsed to int.  The terms are ORed and a term with neither list matches nothing, so it is dropped: () selects no
+    node.  Equal forms select the same nodes.  ValueError naming the owner when a field is malformed, as Kubernetes'
+    validation refuses it (empty or non-list nodeSelectorTerms, an unknown operator, a wrong number of values, a Gt /
+    Lt value that is not an integer, a matchFields key other than metadata.name)."""
+    if affinity is None:
+        return None
+    _mapping(affinity, 'spec.affinity', owner)
+    node = affinity.get('nodeAffinity')
+    if node is None:
+        return None
+    _mapping(node, 'spec.affinity.nodeAffinity', owner)
+    required = node.get('requiredDuringSchedulingIgnoredDuringExecution')
+    if required is None:
+        return None
+    what = 'spec.affinity.nodeAffinity.requiredDuringSchedulingIgnoredDuringExecution'
+    _mapping(required, what, owner)
+    what += '.nodeSelectorTerms'
+    raw = required.get('nodeSelectorTerms')
+    if not isinstance(raw, list) or not raw:
+        raise ValueError("malformed %s of %s: expected a non-empty list, got %r" % (what, owner, raw))
+    terms = set()
+    for t in _entries(raw, what, owner):
+        term = (_node_requirements(t.get('matchExpressions'), what + '.matchExpressions', owner, False),
+                _node_requirements(t.get('matchFields'), what + '.matchFields', owner, True))
+        if term != ((), ()):
+            terms.add(term)
+    return tuple(sorted(terms))
+
+
+class _NewNode(object):
+    """the name (and hostname label) of a node a pool has not created yet: always set, equal to no current node's"""
+
+    def __repr__(self):
+        return '<new node>'
+
+
+NEW_NODE = _NewNode()
+
+
+def requirement_holds(op, values, have):
+    """one NodeSelectorRequirement against a label value or node name `have` (None when the label is absent)"""
+    if op == 'In':
+        return have is not None and have in values
+    if op == 'NotIn':
+        return have is None or have not in values
+    if op == 'Exists':
+        return have is not None
+    if op == 'DoesNotExist':
+        return have is None
+    number = parse_int64(have)  # a missing or non-integer label (and a new node's name) makes Gt / Lt false
+    return number is not None and (number > values[0] if op == 'Gt' else number < values[0])
+
+
+def node_affinity_matches(terms, labels, name):
+    """the canonical required node affinity (node_affinity_terms) admits a node with these labels and this name: no
+    constraint (None), or some term all of whose requirements hold"""
+    if terms is None:
+        return True
+    return any(all(requirement_holds(op, values, labels.get(key)) for key, op, values in exprs) and
+               all(requirement_holds(op, values, name) for _, op, values in fields) for exprs, fields in terms)
+
+
+def pool_affinity_matches(terms, labels):
+    """node_affinity_matches for a new node of a pool with these labels (AgentPool.labels): its name and its
+    kubernetes.io/hostname label are set, to a value no current node has (NEW_NODE), so Exists and NotIn hold there and
+    In, DoesNotExist, Gt and Lt do not.  A pod pinned to existing nodes matches no pool."""
+    return node_affinity_matches(terms, {**labels, HOSTNAME_TOPOLOGY_KEY: NEW_NODE}, NEW_NODE)
+
+
 class KubePodStatus(object):
     RUNNING = 'Running'
     PENDING = 'Pending'
@@ -216,6 +327,7 @@ class KubeResource(object):
 _RESOURCES_MEMO = {}
 _CREATED_BY_MEMO = {}
 _TIME_MEMO = {}
+_AFFINITY_MEMO = {}
 _MISSING = object()
 
 
@@ -317,6 +429,23 @@ class KubePod(object):
     def anti_affinity_terms(self):
         """the honoured required pod anti-affinity terms (kube.anti_affinity_terms); read on use, like tolerations."""
         return anti_affinity_terms(self.original.obj['spec'].get('affinity'), self.namespace, 'pod %s' % self)
+
+    @property
+    def node_affinity(self):
+        """the required node affinity (kube.node_affinity_terms; None when there is none); read on use, like
+        tolerations.  The pods of one controller carry the same affinity, so the parsed form is memoised on the text of
+        the field (JSON values: equal texts are equal fields); a malformed field is not cached and raises on every read."""
+        affinity = self.original.obj['spec'].get('affinity')
+        if affinity is None:
+            return None
+        key = repr(affinity)
+        terms = _AFFINITY_MEMO.get(key, _MISSING)
+        if terms is _MISSING:
+            terms = node_affinity_terms(affinity, 'pod %s' % self)
+            if len(_AFFINITY_MEMO) > (1 << 16):
+                _AFFINITY_MEMO.clear()
+            _AFFINITY_MEMO[key] = terms
+        return terms
 
     def is_mirrored(self):
         daemonset = self._created_by().get('reference', {}).get('kind') == 'DaemonSet'

@@ -67,6 +67,9 @@ class Scaler(object):
         # with node selectors: a pod matches a node or pool only when it also tolerates its blocking taints
         # (Cluster(node_taints=...))
         self.node_taints = False
+        # with node selectors: a pod matches a node or pool only when its required node affinity admits it too
+        # (Cluster(node_affinity=...))
+        self.node_affinity = False
         # required pod anti-affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_anti_affinity=...))
         self.pod_anti_affinity = False
 
@@ -81,7 +84,7 @@ class Scaler(object):
         when every node keeps the reference's "any pod to schedule" rule (the switch is off, or nothing is pending)."""
         if not self.selector_node_states or not pods_to_schedule:
             return None
-        return ~snapshot.pending_match(pods_to_schedule, nodes, taints=self.node_taints)
+        return ~snapshot.pending_match(pods_to_schedule, nodes, taints=self.node_taints, affinity=self.node_affinity)
 
     def get_node_state(self, node, node_pods, pods_to_schedule):
         """ClusterNodeState of one node (scaler.py:61-114): a one-node launch of the idle scan.
@@ -99,7 +102,8 @@ class Scaler(object):
         ordered_pools = capacity.order_by_cost_asc(self.agent_pools)
         classes = None
         if self.node_selectors:
-            classes = snapshot.selector_classes(unique, [], ordered_pools, taints=self.node_taints)
+            classes = snapshot.selector_classes(unique, [], ordered_pools, taints=self.node_taints,
+                                                affinity=self.node_affinity)
         anti_affinity = snapshot.anti_affinity(unique) if self.pod_anti_affinity else None
         res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision,
                                classes=classes, anti_affinity=anti_affinity)

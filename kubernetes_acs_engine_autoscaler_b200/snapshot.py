@@ -170,14 +170,17 @@ def _toleration_items(tolerations):
 class _Projection(object):
     """the nodes grouped by everything a match can see, so that a match is evaluated once per distinct projection,
     vectorised over the projections, instead of once per node.  Each label key in `keys` is read once per node and its
-    values are numbered (a missing label reads as None, as labels.get does in is_match); with `taints`, the node's
-    blocking-taint set (kube.blocking_taints) is numbered as one more column.  `group[n]` is node n's projection."""
+    values are numbered (a missing label reads as None, as labels.get does in is_match); with `names`, the node's name
+    (for matchFields) is numbered as one more column; with `taints`, the node's blocking-taint set
+    (kube.blocking_taints) is numbered as the last column.  `group[n]` is node n's projection."""
 
-    def __init__(self, nodes, keys, taints):
-        codes, self.code_of = [], []  # the number of every node's value per column; per label key: {value: number}
+    def __init__(self, nodes, keys, taints, names=False):
+        codes, self.code_of = [], []  # the number of every node's value per column; per label/name column: {value: number}
         labels = [n.selectors for n in nodes] if keys else []
-        for key in keys:
-            values = [l.get(key) for l in labels]
+        columns = [[l.get(key) for l in labels] for key in keys]
+        if names:
+            columns.append([n.name for n in nodes])
+        for values in columns:
             code = {v: i for i, v in enumerate(dict.fromkeys(values))}
             self.code_of.append(code)
             codes.append(np.fromiter(map(code.__getitem__, values), dtype=np.int64, count=len(values)))
@@ -198,6 +201,43 @@ class _Projection(object):
         self.group = group.reshape(-1)
         self.proj = np.stack([c[first] for c in codes], axis=1) if codes else np.zeros((len(first), 0), np.int64)
         self.column = {key: k for k, key in enumerate(keys)}
+        self.name_column = len(keys) if names else None
+        self._ints = {}
+
+    def _int_table(self, k):
+        """(ok bool[codes], value int64[codes]): the values of column k parsed as kube.parse_int64, per value number"""
+        table = self._ints.get(k)
+        if table is None:
+            parsed = [kube.parse_int64(v) for v in self.code_of[k]]
+            table = self._ints[k] = (np.fromiter((p is not None for p in parsed), dtype=bool, count=len(parsed)),
+                                     np.fromiter((0 if p is None else p for p in parsed), dtype=np.int64,
+                                                 count=len(parsed)))
+        return table
+
+    def _requirement(self, k, op, values):
+        """bool[projections]: the requirement (kube.requirement_holds) on column k"""
+        col, code = self.proj[:, k], self.code_of[k]
+        if op in ('Gt', 'Lt'):
+            ok, number = self._int_table(k)
+            return ok[col] & (number[col] > values[0] if op == 'Gt' else number[col] < values[0])
+        if op in ('Exists', 'DoesNotExist'):
+            op, values = ('NotIn' if op == 'Exists' else 'In'), (None,)
+        hit = np.isin(col, [code[v] for v in values if v in code])
+        return hit if op == 'In' else ~hit
+
+    def affinity(self, terms):
+        """bool[projections]: the canonical required node affinity (kube.node_affinity_terms) admits the nodes"""
+        if terms is None:
+            return np.ones(len(self.proj), dtype=bool)
+        match = np.zeros(len(self.proj), dtype=bool)
+        for exprs, fields in terms:
+            term = np.ones(len(self.proj), dtype=bool)
+            for key, op, values in exprs:
+                term &= self._requirement(self.column[key], op, values)
+            for _, op, values in fields:
+                term &= self._requirement(self.name_column, op, values)
+            match |= term
+        return match
 
     def selector(self, items):
         """bool[projections]: the labels match the selector `items` (KubeNode.is_match)"""
@@ -218,27 +258,51 @@ class _Projection(object):
         return ok[self.proj[:, -1]]
 
 
-def _match_keys(pods, taints):
-    """the distinct (selector items, toleration items) of the pods in first-occurrence order with one toleration list
-    each, and every pod's index into them.  Without taints a pod without a selector gets -1 (it matches everything)."""
+def _match_keys(pods, taints, affinity):
+    """the distinct (selector items, toleration items, canonical node affinity) of the pods in first-occurrence order as
+    (selector items, one toleration list, node affinity), and every pod's index into them.  Without taints a pod without
+    a selector and without a required node affinity gets -1 (it matches everything)."""
     index, distinct = {}, []
     of_pod = np.full(len(pods), -1, dtype=np.int64)
     for i, pod in enumerate(pods):
         selectors = pod.selectors
         tolerations = pod.tolerations if taints else ()
-        if not selectors and not taints:
+        terms = pod.node_affinity if affinity else None
+        if not selectors and not taints and terms is None:
             continue
         key = (tuple(sorted(selectors.items())) if selectors else (),
-               _toleration_items(tolerations) if tolerations else ())
+               _toleration_items(tolerations) if tolerations else (), terms)
         j = index.get(key)
         if j is None:
             j = index[key] = len(distinct)
-            distinct.append((key[0], tolerations))
+            distinct.append((key[0], tolerations, terms))
         of_pod[i] = j
     return distinct, of_pod
 
 
-def selector_classes(pods, nodes, pools, taints=False):
+def _projection(nodes, distinct, taints):
+    """the _Projection of the nodes over every label key the selectors and node-affinity terms read, with the name
+    column when some term has matchFields"""
+    keys, names = set(), False
+    for items, _, terms in distinct:
+        keys.update(key for key, _ in items)
+        for exprs, fields in terms or ():
+            keys.update(key for key, _, _ in exprs)
+            names = names or bool(fields)
+    return _Projection(nodes, sorted(keys), taints, names)
+
+
+def _node_match(proj, items, tolerations, terms, taints):
+    """bool[projections]: selector, node affinity and (with taints) tolerations all admit the nodes"""
+    match = proj.selector(items)
+    if terms is not None:
+        match &= proj.affinity(terms)
+    if taints:
+        match &= proj.tolerated(tolerations)
+    return match
+
+
+def selector_classes(pods, nodes, pools, taints=False, affinity=False):
     """map every distinct match signature (set of matching nodes, set of matching pools) of the pods' nodeSelectors
     to a class number.  Class 0 is "no selector": it matches everything, so a selector that matches every node and
     every pool shares it.  Pods whose selectors match the same nodes and pools share a class.  A pool matches with
@@ -247,23 +311,25 @@ def selector_classes(pods, nodes, pools, taints=False):
     With `taints`, a pod matches a node or pool when its selector matches AND it tolerates every blocking taint there
     (kube.blocking_taints of KubeNode.taints, AgentPool.taints; KubePod.tolerations).  Class 0 keeps its meaning
     (matches every node and pool); it may then have no pod.  Without `taints`, taints and tolerations are never read.
-    Each distinct (selector, tolerations) is evaluated once per distinct node projection (_Projection)."""
+
+    With `affinity`, the pod's required node affinity (KubePod.node_affinity) must admit the node too (a pool: a new
+    node of it, kube.pool_affinity_matches); without it, the field is never read.  Each distinct (selector,
+    tolerations, node affinity) is evaluated once per distinct node projection (_Projection)."""
     pods, nodes, pools = list(pods), list(nodes), list(pools)
-    distinct, of_pod = _match_keys(pods, taints)
+    distinct, of_pod = _match_keys(pods, taints, affinity)
     if not distinct:
         return SelectorClasses(np.zeros(len(pods), dtype=np.uint8), np.ones(len(nodes), dtype=np.uint64),
                                np.ones(len(pools), dtype=np.uint64), 1)
-    proj = _Projection(nodes, sorted({key for items, _ in distinct for key, _ in items}), taints)
+    proj = _projection(nodes, distinct, taints)
     pool_labels = [p.labels for p in pools]
     pool_taints = [p.taints for p in pools] if taints else [()] * len(pools)
     everything = (b"\x01" * len(proj.proj), b"\x01" * len(pools))
     class_of_sig = {everything: 0}
     class_of_key = np.zeros(len(distinct) + 1, dtype=np.uint8)  # the last entry (index -1) is class 0
-    for j, (items, tolerations) in enumerate(distinct):
-        nmatch = proj.selector(items)
-        if taints:
-            nmatch &= proj.tolerated(tolerations)
-        sig = (nmatch.tobytes(), bytes(_selector_matches(l, items) and kube.tolerates_all(tolerations, t)
+    for j, (items, tolerations, terms) in enumerate(distinct):
+        nmatch = _node_match(proj, items, tolerations, terms, taints)
+        sig = (nmatch.tobytes(), bytes(_selector_matches(l, items) and kube.tolerates_all(tolerations, t) and
+                                       kube.pool_affinity_matches(terms, l)
                                        for l, t in zip(pool_labels, pool_taints)))
         c = class_of_sig.get(sig)
         if c is None:
@@ -283,26 +349,26 @@ def selector_classes(pods, nodes, pools, taints=False):
     return SelectorClasses(class_of_key[of_pod], node_match[proj.group], pool_match, len(class_of_sig))
 
 
-def pending_match(pods, nodes, taints=False):
+def pending_match(pods, nodes, taints=False, affinity=False):
     """bool[N]: some pod of `pods` matches node n (KubeNode.is_match).  All True when a pod has no selector.  With
     `taints` a pod matches a node when its selector matches AND it tolerates the node's blocking taints: a pod without
-    a selector then matches only the nodes whose blocking taints it tolerates.
+    a selector then matches only the nodes whose blocking taints it tolerates.  With `affinity` the pod's required node
+    affinity (KubePod.node_affinity) must admit the node too.
 
     Maintain asks this of every node of the scalable pools (up to 10^6), so matches are not evaluated node by node:
-    each distinct (selector, tolerations) is evaluated once per distinct node projection (_Projection)."""
+    each distinct (selector, tolerations, node affinity) is evaluated once per distinct node projection (_Projection)."""
     nodes = list(nodes)
-    if not taints and any(not pod.selectors for pod in pods):
+    if not taints and not affinity and any(not pod.selectors for pod in pods):
         return np.ones(len(nodes), dtype=bool)
-    distinct, _ = _match_keys(pods, taints)
+    distinct, of_pod = _match_keys(pods, taints, affinity)
+    if not taints and (of_pod < 0).any():  # a pod without selector and node affinity
+        return np.ones(len(nodes), dtype=bool)
     if not distinct or not nodes:
         return np.zeros(len(nodes), dtype=bool)
-    proj = _Projection(nodes, sorted({key for items, _ in distinct for key, _ in items}), taints)
+    proj = _projection(nodes, distinct, taints)
     hit = np.zeros(len(proj.proj), dtype=bool)
-    for items, tolerations in distinct:
-        match = proj.selector(items)
-        if taints:
-            match &= proj.tolerated(tolerations)
-        hit |= match
+    for items, tolerations, terms in distinct:
+        hit |= _node_match(proj, items, tolerations, terms, taints)
     return hit[proj.group]
 
 
