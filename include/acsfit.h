@@ -108,7 +108,8 @@ ACSFIT_API acsfit_status acsfit_ctx_destroy(acsfit_ctx *ctx);
 ACSFIT_API acsfit_status acsfit_ctx_configure(acsfit_ctx *ctx, int min_stages, int watchdog_ms);
 /* the same developer knobs by name, after ctx creation: "ranks" (0: float64 compare scan, 1: packed-rank scan when
  * the tick's request table allows it -- the default), "stream" (1: the barrier-free streaming form of the pipeline
- * kernel, csrc/acsfit_stream_ff.cuh, where it applies; env ACSFIT_STREAM), "prune", "overlap", "min_stages", "inject_chain_timeout" (test hook), "cluster_blocks" (cluster
+ * kernel, csrc/acsfit_stream_ff.cuh, where it applies; env ACSFIT_STREAM), "retire" (0: bin passes keep testing
+ * bins that can take no pod of the pass any more; default 1), "prune", "overlap", "min_stages", "inject_chain_timeout" (test hook), "cluster_blocks" (cluster
  * mode: cut the pod list of the node pass into this many blocks; 0 = automatic), and for the K1 / K6 idle scan
  * (csrc/acsfit_scan_plan.h): "bulk_cfg" (geometry of the bulk-copy form, contiguous tables, D <= 8:
  * 0 = 8 KB x 8 warps, 1 = 16 KB x 12, 2 = 16 KB x 8, 3 = 32 KB x 6, anything else = 8 KB x 16, the default 4;

@@ -37,6 +37,7 @@ struct acsfit_ctx {
     int use_stream = 0;       // barrier-free streaming form of the pipeline kernel (acsfit_stream_ff.cuh; ACSFIT_STREAM / knob "stream")
     int use_ranks = 1;        // packed-rank scan when the tick's distinct request values allow it (ACSFIT_RANKS=0: never)
     RankLayout rk;            // rank tables of the current API call (rk.nw == 0: float64 scan)
+    int retire = 1;           // bin passes with rank tables retire bins that can take no pod of the pass (knob "retire")
     // cluster mode (one cluster on `world` GPUs; see include/acsfit.h)
     int rank = 0, world = 1;
     unsigned char *xbase = nullptr;                     // this rank's exchange region (cudaMalloc, IPC-exported)
@@ -853,6 +854,7 @@ extern "C" acsfit_status acsfit_ctx_set_knob(acsfit_ctx *ctx, const char *name, 
     if (!ctx || !name) return ACSFIT_E_INVALID;
     if (!strcmp(name, "ranks")) ctx->use_ranks = value != 0;
     else if (!strcmp(name, "stream")) ctx->use_stream = value != 0;
+    else if (!strcmp(name, "retire")) ctx->retire = value != 0;
     else if (!strcmp(name, "prune")) ctx->prune = value;
     else if (!strcmp(name, "overlap")) ctx->overlap = value != 0;
     else if (!strcmp(name, "min_stages")) ctx->min_stages = std::max(0, value);
@@ -1173,6 +1175,7 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     int held = 0;
     TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA>(ctx, pp, stages, st, &held)));
     q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
+    q.retire = BINS && ctx->retire;
     q.prof = (ctx->prof_dev && stages <= kProfStages) ? ctx->prof_dev : nullptr;
     if (q.prof) {
         CUDA_TRY(cudaMemsetAsync(ctx->prof_dev, 0, sizeof(unsigned long long) * (kProfStages + kProfTiles) * 8, st));

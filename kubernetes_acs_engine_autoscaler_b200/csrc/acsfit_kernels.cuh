@@ -85,6 +85,21 @@ __device__ __forceinline__ uint32_t rank_upper(const double *__restrict__ sorted
     return (uint32_t)lo;
 }
 
+// the same search over a table a bin stage staged in shared memory (see kRankStaged)
+__device__ __forceinline__ uint32_t rank_upper_shared(const double *sorted_d, int U, double thr)
+{
+    int lo = 0, hi = U;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (sorted_d[mid] <= thr) lo = mid + 1; else hi = mid;
+    }
+    return (uint32_t)lo;
+}
+
+// bin stages (RW > 0) copy the sorted values of every dimension with at most this many distinct values into shared
+// memory at stage start: the threshold refresh after each placing tile then searches shared memory, not L2
+constexpr int kRankStaged = 256;
+
 struct PipelineParams {
     // pod side
     const double *req;      // rows of D doubles
@@ -139,6 +154,9 @@ struct PipelineParams {
     const unsigned long long *pod_matches;  // [req rows] terms that select the pod
     unsigned long long *node_carries;       // [N] in/out (node pass)
     unsigned long long *node_matches;       // [N] in/out (node pass)
+    // bin passes with the packed-rank scan (RW > 0; appended): != 0 retires bins that can take no pod of the pass any
+    // more, i.e. S[d] < the smallest request value of dimension d (rk.sorted[d * kRankCap]) in some d
+    int retire;
 };
 
 __device__ __forceinline__ int ld_acquire(const int *p)
@@ -225,7 +243,8 @@ struct PipelineSmem {
                + sizeof(unsigned short) * kTile /*slot_of*/ + (size_t)NW * 32 /*accepted node per dense entry*/
                + sizeof(unsigned) * ((size_t)RW * Tn /*packed node words*/ + (size_t)RW * kTile /*packed pod words*/ + 4 /*alignment*/)
                + (SEL ? sizeof(unsigned long long) * (size_t)Tn /*node masks*/ + kTile /*pod classes*/ + (size_t)NW * 36 /*batch classes*/ : 0)
-               + (AA ? sizeof(unsigned long long) * 2 * ((size_t)Tn /*node carries / matches*/ + kTile /*pod masks*/ + (size_t)NW * 36 /*batch masks*/) : 0);
+               + (AA ? sizeof(unsigned long long) * 2 * ((size_t)Tn /*node carries / matches*/ + kTile /*pod masks*/ + (size_t)NW * 36 /*batch masks*/) : 0)
+               + (BINS && RW > 0 ? sizeof(double) * (size_t)D * (1 /*smallest request*/ + kRankStaged /*staged rank tables*/) : 0);
     }
 };
 
@@ -295,7 +314,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
     unsigned *dirty = opened + NW;                              // [NW] nodes: threshold is stale (bit per node)
     unsigned *wcount = dirty + NW;                              // [8] pods to scan per tile word
     unsigned *acount = wcount + 8;                              // [8] alive pods per tile word
-    unsigned *misc = acount + 8;                                // [8]: 0 stage, 1 abort, 2 drained, 3 any dirty, 4 placed, 5 first candidate
+    unsigned *misc = acount + 8;                                // [8]: 0 stage, 1 abort, 2 drained, 3 any dirty, 4 placed, 5 first candidate, 6 dead warps (bins)
     unsigned *nextw = misc + 8;                                 // [kRing][8] alive words of the next tiles (ring, slot = tile % kRing)
     unsigned *hitlist = nextw + kRing * 8;                      // [kTile+1] ordered hit entries (q+1), then kQueueEnd
     unsigned *queue = hitlist + (kTile + 1);                    // [NW-1][kTile+1] forward queue of warp w -> w+1
@@ -317,6 +336,9 @@ firstfit_pipeline_kernel(const PipelineParams p)
     unsigned long long *px_s = pc_s + kTile;                                                            // [kTile]
     unsigned long long *bc_s = px_s + kTile;                                                            // [NW][36]
     unsigned long long *bx_s = bc_s + NW * 36;                                                          // [NW][36]
+    // bins with the packed-rank scan: the smallest request of each dimension and the staged rank tables
+    double *minreq_s = reinterpret_cast<double *>(AA ? bx_s + NW * 36 : nm_s);  // [D]
+    double *rt_s = minreq_s + D;                                                 // [D][kRankStaged]
 
     const int tid = threadIdx.x;
     const int lane = tid & 31;
@@ -328,6 +350,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
         misc[2] = 0;
         misc[3] = 0;
         misc[4] = 0;
+        if (BINS) misc[6] = 0;
     }
     __syncthreads();
     const int stage = (int)misc[0];
@@ -378,12 +401,26 @@ firstfit_pipeline_kernel(const PipelineParams p)
             nc_s[n] = !BINS && n < n_valid ? p.node_carries[stage_lo + n] : 0ull;
             nx_s[n] = !BINS && n < n_valid ? p.node_matches[stage_lo + n] : 0ull;
         }
+    // Bin retirement (RW > 0).  The rank tables are built over every request row of the call, a superset of the pass's
+    // pods, so sorted[d][0] is a lower bound of every request of the pass in dimension d.  A bin with S[d] < that
+    // bound in some d can take no pod of the pass now, and S only shrinks: it is dead for good.  Without rank tables
+    // (RW == 0, the float64 scan) there is no such bound at hand and nothing retires; retire == 0 turns it off too
+    // (the bound becomes -inf).  A zero bound (a padded dimension) simply retires nothing through that dimension.
+    if constexpr (BINS && RW > 0) {
+        if (tid < D) minreq_s[tid] = p.retire ? __ldg(p.rk.sorted + (size_t)tid * kRankCap) : -__longlong_as_double(0x7FF0000000000000ll);
+        for (int i = tid; i < D * kRankStaged; i += NT) {
+            const int d = i / kRankStaged, k = i - d * kRankStaged;
+            if (p.rk.count[d] <= kRankStaged && k < p.rk.count[d]) rt_s[i] = __ldg(p.rk.sorted + (size_t)d * kRankCap + k);
+        }
+    }
     __syncthreads();
     // (n, d) -> field t' of the node's packed threshold row; callers zero the row first
     auto pack_field = [&](int i) {
         const int d = i / Tn, n = i - d * Tn;
         const double thr = BINS ? state_s[i] : thr_s[i];
-        const uint32_t t = rank_upper(p.rk.sorted + (size_t)d * kRankCap, p.rk.count[d], thr);
+        uint32_t t;
+        if (BINS && p.rk.count[d] <= kRankStaged) t = rank_upper_shared(rt_s + (size_t)d * kRankStaged, p.rk.count[d], thr);
+        else t = rank_upper(p.rk.sorted + (size_t)d * kRankCap, p.rk.count[d], thr);
         atomicOr(&tw_s[n * RW + p.rk.word[d]], t << p.rk.shift[d]);
     };
     if constexpr (RW > 0) {
@@ -527,7 +564,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
         const int64_t j = (int64_t)(p.tile_lo + tile) * kTile + tid;
         const unsigned word = nextw[(tile % kRing) * (kTile / 32) + warp];
         const bool is_alive = (word >> lane) & 1u;
-        bool pass = is_alive;
+        // bins: once every warp of the stage is dead (every bin holds a pod and is too full for the smallest request in
+        // some dimension) the stage can take no pod of any later tile: it forwards every tile untouched
+        const bool retired = BINS && RW > 0 && p.retire && misc[6] == (1u << n_warps) - 1u;
+        bool pass = is_alive && !retired;
         // SEL: the bounds stay resource-only.  A pod they prune exceeds, in some dimension, every threshold of the
         // stage, so it fits no node here whatever the node matches: leaving it out is exact.  A pod that passes
         // only because a node it does not match has room is scanned in vain, which costs time, never a result.
@@ -535,10 +575,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
 #pragma unroll
             for (int d = 0; d < D; ++d) pass = pass & (pre[d] <= smax[d]);
         }
-        const unsigned pword = PRUNE ? __ballot_sync(0xFFFFFFFFu, pass) : word;
+        const unsigned pword = PRUNE ? __ballot_sync(0xFFFFFFFFu, pass) : retired ? 0u : word;
         if (lane == 0 && warp < kTile / 32) {
             wcount[warp] = __popc(pword);
-            if (PRUNE) acount[warp] = __popc(word);
+            if (PRUNE || retired) acount[warp] = __popc(word);
             alive_w[warp] = word;
         }
         if (tid < kTile / 32) hitmask[tid] = 0;
@@ -554,11 +594,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
             const unsigned c = wcount[w];
             base += (w < warp) ? c : 0u;
             total += c;
-            if (PRUNE) alive_total += acount[w];
+            if (PRUNE || retired) alive_total += acount[w];
         }
-        if (!PRUNE) alive_total = total;
+        if (!PRUNE && !retired) alive_total = total;
         if (total == 0) {  // nothing alive, or nothing that could fit here: forward the tile untouched
-            if (PRUNE) forwarded += (long long)alive_total;
+            if (PRUNE || retired) forwarded += (long long)alive_total;
             if (remote_in && warp == 0) {  // the words came from the upstream GPU: this GPU's bitmap must hold them too
                 const int64_t wj = (int64_t)(p.tile_lo + tile) * (kTile / 32) + lane;
                 if (lane < kTile / 32 && wj * 32 < p.M) __stcg(p.alive + wj, alive_w[lane]);
@@ -771,14 +811,21 @@ firstfit_pipeline_kernel(const PipelineParams p)
         if constexpr (SEL) {
             if (tid == 0 && nh && p.sel_hits) atomicAdd(p.sel_hits, (unsigned long long)nh);
         }
+        bool became_dead = false;  // bins: this warp's bins all died in this tile
         if (nh > 0) {
             __syncthreads();
             unsigned out = 0;
             const int first_w = min((int)(misc[5] >> 5), n_warps - 1);
-            if (warp < n_warps && warp >= first_w) {
+            // bins: the chain runs over the live warps at or after first_w only.  A warp reads the queue of the previous
+            // live warp (none: the hit list) and the last live warp forwards nothing.  A dead warp could take no entry
+            // anyway.  The dead bits change only after the barrier at the end of the resolver.
+            const unsigned chain = BINS ? ((1u << n_warps) - 1u) & ~misc[6] & ~((1u << first_w) - 1u) : 0u;
+            const unsigned chain_below = chain & ((1u << warp) - 1u);  // bins: live warps of the chain before this one
+            const bool chain_last = (chain & ~((2u << warp) - 1u)) == 0u;
+            if (BINS ? ((chain >> warp) & 1u) != 0u : warp < n_warps && warp >= first_w) {
                 const int my_lo = warp << 5;
                 const int n = my_lo + lane;
-                const bool last = warp == n_warps - 1;
+                const bool last = BINS ? chain_last : warp == n_warps - 1;
                 double S[D], C[D];
 #pragma unroll
                 for (int d = 0; d < D; ++d) {
@@ -805,7 +852,8 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 }
 
                 unsigned my_takes = 0;  // pods this lane's node / bin took in this tile
-                const volatile unsigned *in_q = warp == first_w ? hitlist : queue + (size_t)(warp - 1) * (kTile + 1);
+                const volatile unsigned *in_q = BINS ? (chain_below ? queue + (size_t)(31 - __clz(chain_below)) * (kTile + 1) : hitlist)
+                                                     : warp == first_w ? hitlist : queue + (size_t)(warp - 1) * (kTile + 1);
                 volatile unsigned *out_q = queue + (size_t)warp * (kTile + 1);
                 unsigned head = 0;
                 int n_placed = 0;
@@ -1022,6 +1070,12 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         touched_or_open |= touched_tile;
                         my_evals += (unsigned long long)ev_local + (unsigned long long)n_placed * (unsigned long long)(stage_lo + my_lo);
                     }
+                    if constexpr (BINS && RW > 0) {  // a bin dies only by taking a pod: the warp's bins are checked here
+                        bool short_d = false;
+#pragma unroll
+                        for (int d = 0; d < D; ++d) short_d = short_d | (S[d] < minreq_s[d]);
+                        became_dead = __all_sync(0xFFFFFFFFu, n >= n_valid || (((touched_or_open >> lane) & 1u) && short_d));
+                    }
                     if (n < Tn) {
 #pragma unroll
                         for (int d = 0; d < D; ++d) state_s[(size_t)d * Tn + n] = S[d];
@@ -1038,10 +1092,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
             }
             __syncthreads();
             // wipe the queue entries this warp wrote so that the next tile starts from "not written"
-            if (warp < n_warps - 1) {
+            if (BINS ? ((chain >> warp) & 1u) && !chain_last : warp < n_warps - 1) {
                 unsigned *out_q = queue + (size_t)warp * (kTile + 1);
                 for (unsigned i = lane; i <= out; i += 32) out_q[i] = 0;
             }
+            if (BINS && became_dead && lane == 0) atomicOr(&misc[6], 1u << warp);  // read from the next tile's (S1) on
         }
         ACSFIT_PROF(3)
         if (PROF_ON && tid == 0) { prof_acc[6] += nh; prof_acc[7] += 1; }

@@ -88,7 +88,7 @@ class Engine(object):
         self._check(self._lib.acsfit_ctx_set_timing(self._ctx, 1 if enabled else 0))
 
     def set_knob(self, name, value):
-        """developer knobs of include/acsfit.h ("ranks", "stream", "prune", "overlap", "min_stages", "cluster_blocks",
+        """developer knobs of include/acsfit.h ("ranks", "stream", "retire", "prune", "overlap", "min_stages", "cluster_blocks",
         "bulk_cfg", "stream_bytes", and the test hooks "inject_chain_timeout", "bin_pass_stages")."""
         self._check(self._lib.acsfit_ctx_set_knob(self._ctx, name.encode(), int(value)))
 
