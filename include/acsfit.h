@@ -469,6 +469,14 @@ ACSFIT_API acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out
  * call without a selector node pass */
 ACSFIT_API acsfit_status acsfit_last_sel_hits(const acsfit_ctx *ctx, uint64_t *out);
 
+/* test hook (read-only): what bin retirement marked in the last API call's bin passes (barrier form with rank tables,
+ * the chained first pass of scale_up included; in cluster mode this rank's stages only):
+ *   out[0] = resolver warps whose 32 bins were all dead when their stage exited, summed over stages and passes,
+ *   out[1] = stages whose warps were all dead at exit.
+ * A warp is dead when every bin of it holds a pod and is below the call's smallest request in some dimension.  Both are
+ * 0 after a call without such a pass, with knob "retire" = 0, or for passes that hit the watchdog. */
+ACSFIT_API acsfit_status acsfit_last_bin_retirement(const acsfit_ctx *ctx, uint64_t out[2]);
+
 /* developer probes (tools/perf_probe.py): per-stage clock64 phase totals [stages][8] of the last
  * pipeline launch (wait, load, scan, resolve, publish, refresh, hits, tiles) and a per-tile trace
  * [tiles][8] of one chosen stage.  Enabling them adds a clock read per phase on thread 0. */

@@ -47,6 +47,7 @@ SIGNATURES = {
     "acsfit_last_launches": (c_int, [c_vp, c_vp, c_int, c_vp]),
     "acsfit_last_scan_launch": (c_int, [c_vp, c_vp]),
     "acsfit_last_sel_hits": (c_int, [c_vp, c_vp]),
+    "acsfit_last_bin_retirement": (c_int, [c_vp, c_vp]),
     # node selectors: the arguments of the plain form plus a `const acsfit_selectors *` (Selectors below)
     "acsfit_feasible_mask_sel": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
     "acsfit_first_fit_nodes_sel": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,

@@ -51,6 +51,8 @@ struct acsfit_ctx {
     int bin_pass_stages = 0;                            // test knob: at most this many stages per bin pass (0: kMaxStagesPerPass)
     int chain_fallbacks = 0;                            // chained nodes+bins launches that hit the watchdog and were redone unchained
     uint64_t last_sel_hits = 0;                         // hit entries of the selector node passes of the last call (acsfit_last_sel_hits)
+    unsigned long long *retire_dev = nullptr;           // [2] dead warps / retired stages of the last call's bin passes
+    bool retire_counted = false;                        // retire_dev was zeroed by a bin pass of the last call (acsfit_last_bin_retirement)
     // launch records of the current API call (acsfit_last_launches); rec_* are set by the caller of a pipeline launch
     std::vector<std::array<int, ACSFIT_LAUNCH_FIELDS>> launch_log;
     int rec_chained = 0, rec_pool = -1;
@@ -814,7 +816,8 @@ extern "C" acsfit_status acsfit_ctx_create(int device, acsfit_ctx **out_ctx)
     if (const char *env = getenv("ACSFIT_TRACE")) g_trace = atoi(env);
     if (cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming) != cudaSuccess ||
+        cudaMalloc(&ctx->retire_dev, 2 * sizeof(unsigned long long)) != cudaSuccess) {
         delete ctx;
         return ACSFIT_E_CUDA;
     }
@@ -832,6 +835,7 @@ extern "C" acsfit_status acsfit_ctx_destroy(acsfit_ctx *ctx)
         if (ctx->peer[r] && ctx->peer[r] != ctx->xbase) cudaIpcCloseMemHandle(ctx->peer[r]);
     if (ctx->xbase) cudaFree(ctx->xbase);
     if (ctx->prof_dev) cudaFree(ctx->prof_dev);
+    if (ctx->retire_dev) cudaFree(ctx->retire_dev);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
@@ -941,6 +945,18 @@ extern "C" acsfit_status acsfit_last_sel_hits(const acsfit_ctx *ctx, uint64_t *o
     return ACSFIT_OK;
 }
 
+extern "C" acsfit_status acsfit_last_bin_retirement(const acsfit_ctx *ctx, uint64_t out[2])
+{
+    if (!ctx || !out) return ACSFIT_E_INVALID;
+    out[0] = out[1] = 0;
+    if (!ctx->retire_counted) return ACSFIT_OK;
+    // every bin pass of the call has finished: the entry points synchronise before they return
+    if (cudaSetDevice(ctx->device) != cudaSuccess ||
+        cudaMemcpy(out, ctx->retire_dev, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return ACSFIT_E_CUDA;
+    return ACSFIT_OK;
+}
+
 extern "C" acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out)
 {
     static_assert(sizeof(ScanLaunch) == sizeof(int) * ACSFIT_SCAN_FIELDS, "one int per record field");
@@ -974,6 +990,7 @@ static acsfit_status enter(acsfit_ctx *ctx, int D)
     ctx->scan_rec = ScanLaunch{};
     ctx->rec_chained = 0;
     ctx->rec_pool = -1;
+    ctx->retire_counted = false;  // (reset_stats clears it too: the redo of a timed-out chained launch)
     return ACSFIT_OK;
 }
 
@@ -1176,6 +1193,11 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA>(ctx, pp, stages, st, &held)));
     q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
     q.retire = BINS && ctx->retire;
+    if (BINS && RW > 0) {  // the first counted bin pass of a call zeroes the counters (in stream order before the later ones)
+        if (!ctx->retire_counted) CUDA_TRY(cudaMemsetAsync(ctx->retire_dev, 0, 2 * sizeof(unsigned long long), st));
+        ctx->retire_counted = true;
+        q.retire_count = ctx->retire_dev;
+    }
     q.prof = (ctx->prof_dev && stages <= kProfStages) ? ctx->prof_dev : nullptr;
     if (q.prof) {
         CUDA_TRY(cudaMemsetAsync(ctx->prof_dev, 0, sizeof(unsigned long long) * (kProfStages + kProfTiles) * 8, st));
@@ -1656,6 +1678,7 @@ static void reset_stats(acsfit_ctx *ctx)
     ctx->last_decisions = 0;
     ctx->last_stages = ctx->last_tiles = 0;
     ctx->last_sel_hits = 0;
+    ctx->retire_counted = false;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -157,6 +157,9 @@ struct PipelineParams {
     // bin passes with the packed-rank scan (RW > 0; appended): != 0 retires bins that can take no pod of the pass any
     // more, i.e. S[d] < the smallest request value of dimension d (rk.sorted[d * kRankCap]) in some d
     int retire;
+    // bin passes with the packed-rank scan (appended; test hook acsfit_last_bin_retirement): [0] += warps whose bins
+    // were all dead when their stage exited, [1] += stages whose warps were all dead.  nullptr: not counted
+    unsigned long long *retire_count;
 };
 
 __device__ __forceinline__ int ld_acquire(const int *p)
@@ -1183,6 +1186,17 @@ firstfit_pipeline_kernel(const PipelineParams p)
         if (forwarded == 0) atomicExch(p.drained, 1);
         if (PROF_ON) {
             for (int i = 0; i < 8; ++i) p.prof[(size_t)stage * 8 + i] = prof_acc[i];
+        }
+    }
+    // misc[6] is final: its last atomicOr precedes the barrier above.  The stage's warp count is recomputed from the
+    // parameters and misc[0] so that no register stays live across the tile loop for it.
+    if constexpr (BINS && RW > 0) {
+        if (tid == 0 && p.retire_count && misc[6]) {
+            const unsigned dead = misc[6];
+            const int64_t lo = p.node_lo + (int64_t)misc[0] * p.Tn;
+            const int nw = (int)((max((int64_t)0, min((int64_t)p.Tn, p.node_hi - lo)) + 31) >> 5);
+            atomicAdd(p.retire_count, (unsigned long long)__popc(dead));
+            if (dead == (1u << nw) - 1u) atomicAdd(p.retire_count + 1, 1ull);
         }
     }
 }

@@ -163,6 +163,13 @@ class Engine(object):
         self._check(self._lib.acsfit_last_sel_hits(self._ctx, ctypes.cast(ctypes.byref(out), ctypes.c_void_p)))
         return int(out.value)
 
+    def last_bin_retirement(self):
+        """test hook: (dead warps, retired stages) that bin retirement marked in the last call's bin passes (barrier form
+        with rank tables; summed over stages and passes; in cluster mode this rank's stages)."""
+        out = np.zeros(2, dtype=np.uint64)
+        self._check(self._lib.acsfit_last_bin_retirement(self._ctx, _ptr(out)))
+        return int(out[0]), int(out[1])
+
     def debug_profile(self, enabled=True):
         """developer probe: per-stage clock64 totals [stages, 8] of the last pipeline launch
         (wait, load, scan, resolve, publish, refresh, hits, tiles)."""

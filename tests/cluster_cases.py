@@ -11,6 +11,7 @@ tests/test_gpu_cluster.py runs them.
 """
 import numpy as np
 
+import bin_chain_cases as bcc
 import variant_cases as vc
 from kubernetes_acs_engine_autoscaler_b200 import synthetic as syn
 
@@ -166,6 +167,22 @@ def closed_form_answer(M, take):
 
 
 CLOSED_SMALL = (600, 400)   # (M, take) of the first, single-pass closed-form call
+RETIRE_STAGES = 40          # stages per rank of the retiring bin pass (retire_input)
+
+
+def retire_input(world, tn, S=RETIRE_STAGES):
+    """fulfill_pending input whose single cluster bin pass has S stages of tn bins on every rank (world * S * tn pods,
+    one pool, D = 4).  Openers of 8 in a unit of 10 fill every bin of rank 0 and of rank 1's stage 0 (2 left: dead, the
+    call's minimum is 3), so rank 1's stage 0 retires in the tile of its last opener and passes every later tile on,
+    copying the alive words it gets from rank 0 into rank 1's bitmap; the rest (big pods of 9 and probes of 3,
+    tests/bin_chain_cases.py) places on rank 1's later stages and on the next ranks"""
+    M = world * S * tn
+    n_open = S * tn + tn
+    rest = M - n_open
+    col = [bcc.DEAD] * n_open + bcc.tail(rest // 3, rest - rest // 3)
+    req = bcc.rows(col, 4)
+    return {"req": req, "num_listed": M, "unit": bcc.unit_row(4).reshape(1, -1), "pool_actual": np.zeros(1, np.int32),
+            "pool_max": np.array([1 << 30], np.int32), "pool_ignored": np.zeros(1, np.uint8), "over_provision": 0}
 
 
 def closed_full(world, resident, tn):
@@ -176,7 +193,8 @@ def closed_full(world, resident, tn):
 
 # name -> (builder(world, sms), calls, knobs, in the reduced list of worlds 3 and 4)
 # calls: "scale_up", "scale_up_host", "ff_all" (first_fit_nodes over every row, pod_idx None), "ff_subset" (the
-# tick's sorted pod_idx), "fulfill" (the tick's fulfill input), "closed" (the multi-pass closed form)
+# tick's sorted pod_idx), "fulfill" (the tick's fulfill input), "closed" (the multi-pass closed form), "retire" (a
+# bin pass in which a stage of rank 1 retires, retire_input sized from a small first call's stage width)
 CASES = {}
 
 
@@ -224,11 +242,15 @@ _add("fulfill_d8", lambda w, s: _fulfill(8, 51), ("fulfill",))
 _add("fulfill_d16", lambda w, s: _fulfill(16, 52), ("fulfill",))
 _add("bins_closed_d16", lambda w, s: {"D": 16, "N": 0}, ("closed",), reduced=True)
 
+# bin retirement: rank 1's stage 0 retires while later stages place (and once with retirement off)
+_add("retire_rank1", lambda w, s: {"D": 4, "N": 0}, ("retire",), reduced=True)
+_add("retire_rank1_off", lambda w, s: {"D": 4, "N": 0}, ("retire",), {"retire": 0}, reduced=True)
+
 
 def oracle_call(oracle, c, call):
     """the oracle's answer to one call on tick c (every rank must return exactly this)"""
-    if call == "closed":
-        raise ValueError("the closed-form calls are answered by closed_form_answer")
+    if call in ("closed", "retire"):
+        raise ValueError("the %s calls are sized on the GPU: answer them with their input" % call)
     if call == "fulfill":
         f = c["fulfill"]
         return oracle.fulfill_pending(f["req"], f["num_listed"], f["unit"], f["pool_actual"], f["pool_max"],

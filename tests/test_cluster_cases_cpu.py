@@ -25,7 +25,7 @@ def test_case_lists():
     assert {"layout_" + n for n in vc.LAYOUTS} <= set(cc.CASES)
     for name in cc.CASES:
         for call in cc.calls(name):
-            assert call in ("scale_up", "scale_up_host", "ff_all", "ff_subset", "fulfill", "closed"), (name, call)
+            assert call in ("scale_up", "scale_up_host", "ff_all", "ff_subset", "fulfill", "closed", "retire"), (name, call)
 
 
 @pytest.mark.parametrize("name", sorted(n for n in cc.CASES if n.startswith("layout_")))
@@ -140,3 +140,29 @@ def test_closed_form_equals_oracle(oracle_mod, D):
     M, take = cc.closed_full(2, cc.H100_SMS, cc.MIN_TN)
     first = 2 * cc.H100_SMS * cc.MIN_TN
     assert first < take < M < 2 * first  # pool 0 is cut inside the second pass
+
+
+@pytest.mark.parametrize("world", WORLDS)
+def test_retire_case(oracle_mod, world):
+    """rank 0's bins and rank 1's stage 0 are all dead, rank 1's stage 0 dies inside the pass (later tiles follow),
+    and the pods after it are placed on rank 1's later stages and, with three ranks or more, on rank 2"""
+    import bin_chain_cases as bcc
+    tn, S = cc.MIN_TN, cc.RETIRE_STAGES
+    f = cc.retire_input(world, tn)
+    M = f["req"].shape[0]
+    assert -(-(-(-M // tn)) // world) == S  # the cluster plan: S stages of tn bins per rank
+    o = oracle_mod.fulfill_pending(f["req"], f["num_listed"], f["unit"], f["pool_actual"], f["pool_max"],
+                                   f["pool_ignored"], f["over_provision"])
+    assert (o["bin_of"] >= 0).all() and o["bins_opened"][0] <= M  # one pass
+    Sb = bcc.remaining(f["req"], o["bin_of"], f["unit"][0])
+    mr = bcc.minreq(f["req"])
+    assert all(bcc.stage_dead_mask(Sb, mr, s * tn, tn) == 1 for s in range(S + 1))
+    last_opener = S * tn + tn - 1
+    assert last_opener // cc.TILE < (M - 1) // cc.TILE  # tiles come after the stage retired
+    rank1 = o["bin_of"][last_opener + 1:]
+    assert (rank1 < world * S * tn).all() and ((rank1 >= (S + 1) * tn) & (rank1 < 2 * S * tn)).sum() > 100
+    if world >= 3:
+        assert (rank1 >= 2 * S * tn).sum() > 100
+    rec = [{"pass": 1, "RW": 1, "form": 0, "Tn": tn, "stages": S, "pool": 0, "bin_base": 0}]
+    per_rank = [bcc.retirement(rec, {0: Sb}, mr, rank=r) for r in range(world)]
+    assert per_rank[0] == (S, S) and per_rank[1][1] >= 1

@@ -25,6 +25,7 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
+import bin_chain_cases as bcc
 import cluster_cases as cc
 import variant_cases as vc
 from test_rank_math_cpu import layout
@@ -35,7 +36,7 @@ pytestmark = pytest.mark.gpu
 MODES = ("ranks", "f64", "stream")
 SESSIONS = {"w2": (2, "gloo"), "w3": (3, "gloo"), "w4": (4, "gloo"), "w2_nccl": (2, "nccl")}
 JOIN_TIMEOUT_S = 900
-DEFAULT_KNOBS = {"cluster_blocks": 0, "prune": -1, "bin_pass_stages": 0}
+DEFAULT_KNOBS = {"cluster_blocks": 0, "prune": -1, "bin_pass_stages": 0, "retire": 1}
 # the small exchange region the refusals are checked on
 REF_PODS, REF_NODES, REF_DIMS = 600, 200, 8
 REFUSALS = ("scale_up_sel", "first_fit_nodes_sel", "fulfill_pending_sel", "ff_pods_over", "ff_nodes_over",
@@ -104,7 +105,7 @@ def _run_call(eng, c, call, knobs):
     else:
         if call == "fulfill":
             f = c["fulfill"]
-        else:  # closed: a small single-pass call first, then one sized from its launch records
+        else:  # closed / retire: a small single-pass call first, then one sized from its launch records
             f = cc.closed_form_input(*cc.CLOSED_SMALL, c["D"])
         g = eng.fulfill_pending(eng.dev(f["req"], f64), f["num_listed"], f["unit"], f["pool_actual"], f["pool_max"],
                                 f["pool_ignored"], f["over_provision"])
@@ -117,10 +118,18 @@ def _run_call(eng, c, call, knobs):
             g = eng.fulfill_pending(eng.dev(f["req"], f64), M, f["unit"], f["pool_actual"], f["pool_max"],
                                     f["pool_ignored"], f["over_provision"])
             out["closed"] = np.array([M, take, small["resident"], small["Tn"]])
+        if call == "retire":
+            torch.cuda.synchronize()
+            small = [r for r in eng.last_launches() if r["pass"] == 1 and r["pool"] == 0][0]
+            f = cc.retire_input(eng.cluster_world, small["Tn"])
+            g = eng.fulfill_pending(eng.dev(f["req"], f64), f["num_listed"], f["unit"], f["pool_actual"],
+                                    f["pool_max"], f["pool_ignored"], f["over_provision"])
+            out["retire"] = np.array([small["Tn"]])
         torch.cuda.synchronize()
         for k, v in g.items():
             out[k] = v.cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
     out["rec"] = np.array([[r[k] for k in _launch_fields()] for r in eng.last_launches()], np.int32).reshape(-1, 12)
+    out["hook"] = np.array(eng.last_bin_retirement(), np.int64)
     p = eng.cluster_last_plan()
     out["plan"] = np.array([p["stage_nodes"], p["stages"], p["pod_blocks"], p["resident"]], np.int32)
     return out
@@ -317,7 +326,43 @@ def tick_and_oracle(name, world, sms, i):
     import oracle
     c = cc.build(name, world, sms)
     call = cc.calls(name)[i]
-    return c, (None if call == "closed" else cc.oracle_call(oracle, c, call))
+    return c, (None if call in ("closed", "retire") else cc.oracle_call(oracle, c, call))
+
+
+@functools.lru_cache(maxsize=None)
+def bins_and_min(name, world, sms, i, size):
+    """(each pool's final bins, the call's smallest request per dimension) of one call, from the oracle; size: (M, take)
+    of a closed-form call, (tn,) of a retire call.  A pool's bins come from the oracle packing the pods that reached
+    it into that pool alone (tests/bin_chain_cases.py)."""
+    import oracle
+    c, o = tick_and_oracle(name, world, sms, i)
+    call = cc.calls(name)[i]
+    if call in ("ff_all", "ff_subset"):
+        return {}, None
+    if call in ("scale_up", "scale_up_host"):
+        pend = np.nonzero(o["placed"] == -1)[0]
+        rows, acc, all_rows = c["req"][pend], o["acc_pool"][pend], c["req"]
+        unit, ignored = c["unit_ordered"], c["pool_ignored"]
+    else:
+        f = {"fulfill": lambda: c["fulfill"], "closed": lambda: cc.closed_form_input(*size, c["D"]),
+             "retire": lambda: cc.retire_input(world, *size)}[call]()
+        full = oracle.fulfill_pending(f["req"], f["num_listed"], f["unit"], f["pool_actual"], f["pool_max"],
+                                      f["pool_ignored"], f["over_provision"])
+        rows, acc, all_rows, unit, ignored = f["req"], full["acc_pool"], f["req"], f["unit"], f["pool_ignored"]
+
+    def one(t, idx):
+        return oracle.fulfill_pending(rows[idx], len(idx), unit[t:t + 1], np.zeros(1, np.int32),
+                                      np.array([1 << 30], np.int32), np.zeros(1, np.uint8), 0)["bin_of"]
+    return bcc.pool_bins(one, rows, acc, unit, ignored), bcc.minreq(all_rows)
+
+
+def check_retirement(g, recs, name, world, sms, i, rank, knobs, size):
+    """this rank's report of what bin retirement marked (dead warps, retired stages of its own stages) against the model
+    over the oracle's bins; (0, 0) for calls without a bin pass and with retirement off"""
+    S, mr = bins_and_min(name, world, sms, i, size)
+    want = (0, 0) if mr is None or not knobs.get("retire", 1) else bcc.retirement(recs, S, mr, rank=rank)
+    assert tuple(int(v) for v in g["hook"]) == want, ("hook (dead warps, retired stages)", tuple(g["hook"]), want)
+    return want
 
 
 def expected_rw(rows, mode):
@@ -329,6 +374,14 @@ def expected_rw(rows, mode):
 def records(g):
     from kubernetes_acs_engine_autoscaler_b200 import _native
     return [dict(zip(_native.LAUNCH_FIELDS, (int(v) for v in row))) for row in g["rec"]]
+
+
+@functools.lru_cache(maxsize=None)
+def retire_oracle(world, tn):
+    import oracle
+    f = cc.retire_input(world, tn)
+    return oracle.fulfill_pending(f["req"], f["num_listed"], f["unit"], f["pool_actual"], f["pool_max"],
+                                  f["pool_ignored"], f["over_provision"])
 
 
 def check_result(g, o, call):
@@ -358,8 +411,8 @@ def check_plan(g, c, call, knobs, world, rank, mode, rw, node_pods, bins_opened)
     for r in recs:
         assert r["chained"] == 0 and r["D"] == D and r["RW"] == rw, r
     nodes = [r for r in recs if r["pass"] == 0]
-    N = c["node_type"].shape[0] if call != "fulfill" and call != "closed" else 0
-    if call in ("fulfill", "closed") or node_pods == 0 or N == 0:
+    N = c["node_type"].shape[0] if call not in ("fulfill", "closed", "retire") else 0
+    if call in ("fulfill", "closed", "retire") or node_pods == 0 or N == 0:
         assert not nodes, recs
     else:
         assert tn in (32, 64, 128, 256) and tn <= cc.max_stage_nodes(D), g["plan"]
@@ -411,23 +464,39 @@ def test_cluster_case(out_root, sid, mode, name):
     knobs = cc.knobs(name)
     for i, call in enumerate(cc.calls(name)):
         c, o = tick_and_oracle(name, world, sms, i)
+        reports = []
         for rank in range(world):
             g = load(s, "%s__%s__%d" % (mode, name, i), rank)
+            size = ()
             if call == "closed":
                 M, take, resident, tn = (int(v) for v in g["closed"])
                 o = cc.closed_form_answer(M, take)
                 assert tn == cc.MIN_TN, g["closed"]
                 rows = cc.closed_form_input(M, take, c["D"])["req"]
+                size = (M, take)
+            elif call == "retire":
+                tn = int(g["retire"][0])
+                assert tn == cc.MIN_TN, g["retire"]
+                f = cc.retire_input(world, tn)
+                o = retire_oracle(world, tn)
+                rows = f["req"]
+                size = (tn,)
             elif call == "fulfill":
                 rows = c["fulfill"]["req"]
             else:
                 rows = c["req"]
             try:
-                check_result(g, o, "fulfill" if call == "closed" else call)
+                check_result(g, o, "fulfill" if call in ("closed", "retire") else call)
                 node_pods = {"ff_all": rows.shape[0], "ff_subset": len(c.get("pod_idx", ())),
                              "scale_up": o.get("n_to_schedule", 0), "scale_up_host": o.get("n_to_schedule", 0)}
                 recs, plan = check_plan(g, c, call, knobs, world, rank, mode, expected_rw(rows, mode),
                                         node_pods.get(call, 0), o.get("bins_opened", ()))
+                reports.append(check_retirement(g, recs, name, world, sms, i, rank, knobs, size))
+                if call == "retire":  # one pass of RETIRE_STAGES stages per rank; rank 1's stage 0 retired in it
+                    bins = [r for r in recs if r["pass"] == 1]
+                    assert [(r["stages"], r["Tn"], r["bin_base"]) for r in bins] == [(cc.RETIRE_STAGES, tn, 0)], bins
+                    if rank == 1 and knobs.get("retire", 1) and bins[0]["RW"] > 0 and bins[0]["form"] == 0:
+                        assert reports[-1][1] >= 1, reports[-1]
                 if name == "blocks_auto":
                     assert not knobs and plan[2] > 1 and plan[1] > plan[3], plan  # waves: blocks chosen by the library
                 if call == "closed":
@@ -437,6 +506,8 @@ def test_cluster_case(out_root, sid, mode, name):
                     assert pool0[1]["bin_base"] == world * resident * tn
             except AssertionError as e:
                 raise AssertionError("%s / %s call %d (%s), rank %d of %d: %s" % (mode, name, i, call, rank, world, e))
+        if call == "retire" and knobs.get("retire", 1) and mode == "ranks":
+            assert sum(r[1] for r in reports) > 0, reports  # the ranks together retired stages
 
 
 @pytest.mark.parametrize("sid", list(SESSIONS))

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import bin_chain_cases as bcc
 from kubernetes_acs_engine_autoscaler_b200 import synthetic as syn
 from test_gpu_parity import bits, oracle_scale_up, to_np
 
@@ -14,18 +15,37 @@ pytestmark = pytest.mark.gpu
 
 
 def test_c2_full_tick_matches_oracle(engine, oracle_mod):
+    """the c2 tick, exactly against the oracle with bin retirement on and off.  Its bin pass opens about 30 k bins,
+    almost all of them dead by the end: what retirement reports (dead warps, retired stages) must equal the model of
+    tests/bin_chain_cases.py over the oracle's bins, and be nearly every warp of the pass"""
     c = syn.make_cluster(100000, 10000, 4, 1, seed=20260923)
     used0 = syn.initial_used(c)
     used_o = used0.copy()
     o = oracle_scale_up(oracle_mod, c, used_o)
-    used_h = used0.copy()
-    h = engine.scale_up_host(c["req"], c["unit_all"], c["unit_ordered"], c["pool_actual"], c["pool_max"],
-                             c["pool_ignored"], c["over_provision"], c["cap_type"], c["node_type"], used_h)
-    for k in ("feasible", "placed", "acc_pool", "new_size", "units_needed", "bins_opened"):
-        np.testing.assert_array_equal(h[k], o[k], err_msg=k)
-    for k in ("n_to_schedule", "n_pending", "num_unaccounted", "decisions"):
-        assert h[k] == o[k], k
-    np.testing.assert_array_equal(bits(used_h), bits(used_o))
+    pend = np.nonzero(o["placed"] == -1)[0]
+    f = oracle_mod.fulfill_pending(c["req"][pend], len(pend), c["unit_ordered"], c["pool_actual"], c["pool_max"],
+                                   c["pool_ignored"], c["over_provision"])
+    S = {0: bcc.remaining(c["req"][pend], f["bin_of"], c["unit_ordered"][0])}
+    assert len(S[0]) == o["bins_opened"][0] > 25000
+    try:
+        for retire in (1, 0):
+            engine.set_knob("retire", retire)
+            used_h = used0.copy()
+            h = engine.scale_up_host(c["req"], c["unit_all"], c["unit_ordered"], c["pool_actual"], c["pool_max"],
+                                     c["pool_ignored"], c["over_provision"], c["cap_type"], c["node_type"], used_h)
+            for k in ("feasible", "placed", "acc_pool", "new_size", "units_needed", "bins_opened"):
+                np.testing.assert_array_equal(h[k], o[k], err_msg="%s (retire=%d)" % (k, retire))
+            for k in ("n_to_schedule", "n_pending", "num_unaccounted", "decisions"):
+                assert h[k] == o[k], (k, retire)
+            np.testing.assert_array_equal(bits(used_h), bits(used_o))
+            recs = engine.last_launches()
+            got = engine.last_bin_retirement()
+            want = bcc.retirement(recs, S, bcc.minreq(c["req"])) if retire else (0, 0)
+            assert got == want, (retire, got, want, [r for r in recs if r["pass"] == 1])
+            if retire and all(r["RW"] > 0 and r["form"] == 0 for r in recs if r["pass"] == 1):
+                assert got[0] > 0.9 * len(S[0]) / 32, got  # nearly every warp over the opened bins is dead
+    finally:
+        engine.set_knob("retire", 1)
     assert o["decisions"] > 1.5e9  # the configuration the metric is quoted on
 
 
