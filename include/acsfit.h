@@ -222,6 +222,31 @@ ACSFIT_API acsfit_status acsfit_node_states(acsfit_ctx *ctx, const int64_t *row_
                                  uint8_t *out_state, acsfit_stream_t stream);
 
 /*
+ * Pending-pod admission with required pod anti-affinity (opt-in): sets ACSFIT_NODEF_NO_PENDING_MATCH on every node
+ * that no pod to schedule could land on, for acsfit_node_states.  NC(n) / NX(n) are the OR of the carries / matches
+ * masks (acsfit_anti_affinity's term numbering) over the pods already on node n.  A signature (class c, carries,
+ * matches) admits node n when bit c of node_match[n] is set and (carries & NX(n)) | (matches & NC(n)) == 0, the
+ * scheduler's block test in both directions.  The host passes the DISTINCT signatures of the pods to schedule, so a
+ * node admits some pod to schedule exactly when some signature admits it.  A node no signature admits gains the flag
+ * bit; every other bit of node_flags_inout is left as it is.  A node with no pods is blocked by nothing.
+ *   row_ptr     [dev] N+1 int64: the pods of node n are rows row_ptr[n] .. row_ptr[n+1] of the run masks (absolute
+ *               row numbers: row_ptr[0] may be > 0); this is the contiguous node-order table of acsfit_node_states
+ *   run_carries, run_matches [dev] one mask per row (may be NULL when row_ptr[N] == row_ptr[0])
+ *   node_match  [dev] N class masks as in acsfit_selectors, or NULL: every node matches every class
+ *   sig_class   [host] U bytes, each < ACSFIT_MAX_CLASSES; sig_carries, sig_matches [host] U masks each
+ *   node_flags_inout [dev] N bytes (ACSFIT_NODEF_*)
+ * U may be 0 (every node gains the flag) and has no upper bound: the kernel stages the table through shared memory
+ * in tiles.  row_ptr and the [dev] masks must be 8-byte aligned.  ACSFIT_E_INVALID: N < 0, U < 0, a class >= 64, a
+ * NULL array that is read, a misaligned array, or row_ptr[N] < row_ptr[0].  The call synchronises the stream (the
+ * table is a host buffer).  acsfit_last_scan_launch reports the launch as kernel 3.
+ */
+ACSFIT_API acsfit_status acsfit_pending_admit(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
+                                              const uint64_t *run_matches, int64_t N, const uint64_t *node_match,
+                                              const uint8_t *sig_class, const uint64_t *sig_carries,
+                                              const uint64_t *sig_matches, int U, uint8_t *node_flags_inout,
+                                              acsfit_stream_t stream);
+
+/*
  * K6b maintain_actions -- the decision part of EngineScaler.maintain (reference
  * engine_scaler.py:133-182): SPARE_AGENT substitution against the per-pool drain budget
  * (budget0 = actual - len(unschedulable) - spare, :136; it only decrements when not dry_run,
@@ -460,7 +485,8 @@ ACSFIT_API acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, i
  * launched, one record of ACSFIT_SCAN_FIELDS ints written to out:
  *   {kernel (0 none, 1 occupancy, 2 node states), form (0 per thread, 1 index gather, 2 bulk copy), D,
  *    staging bytes per warp (0 per thread), warps per CTA, table entries per staging chunk (0 per thread),
- *    grid (CTAs), S (idle thresholds; 0 for occupancy)} */
+ *    grid (CTAs), S (idle thresholds; 0 for occupancy)}
+ * acsfit_pending_admit reports {3, 0, 0, shared-memory bytes per CTA, warps per CTA, signatures per tile, grid, U}. */
 #define ACSFIT_SCAN_FIELDS 8
 ACSFIT_API acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out);
 

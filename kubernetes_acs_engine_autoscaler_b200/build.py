@@ -13,7 +13,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libacsfit.so")
 SOURCES = ["acsfit.cu"]
-HEADERS = ["acsfit_kernels.cuh", "acsfit_math.cuh", "acsfit_rank.cuh", "acsfit_scan_plan.h", "acsfit_stream.cuh", "acsfit_stream_ff.cuh", os.path.join("..", "..", "include", "acsfit.h")]
+HEADERS = ["acsfit_admit.cuh", "acsfit_kernels.cuh", "acsfit_math.cuh", "acsfit_rank.cuh", "acsfit_scan_plan.h", "acsfit_stream.cuh", "acsfit_stream_ff.cuh", os.path.join("..", "..", "include", "acsfit.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

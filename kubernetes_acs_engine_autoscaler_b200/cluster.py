@@ -55,7 +55,7 @@ class Cluster(object):
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
-                 node_taints=None, pod_anti_affinity=None, node_affinity=None):
+                 node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -91,6 +91,14 @@ class Cluster(object):
         if pod_anti_affinity is None:
             pod_anti_affinity = os.environ.get('ACSFIT_POD_ANTI_AFFINITY', '0') not in ('', '0')
         self.pod_anti_affinity = bool(pod_anti_affinity)
+        # with pod anti-affinity on, also in maintain: a node is pod-pending only when some pod to schedule could land on
+        # it given the pods already there, so a pending replica does not freeze the nodes that run its siblings
+        # (opt-in; None: $ACSFIT_ANTI_AFFINITY_NODE_STATES).  With selector_node_states on, both rules apply.
+        if anti_affinity_node_states is None:
+            anti_affinity_node_states = os.environ.get('ACSFIT_ANTI_AFFINITY_NODE_STATES', '0') not in ('', '0')
+        elif anti_affinity_node_states and not self.pod_anti_affinity:
+            raise ValueError("anti_affinity_node_states=True needs pod_anti_affinity on")
+        self.anti_affinity_node_states = bool(anti_affinity_node_states) and self.pod_anti_affinity
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -192,7 +200,8 @@ class Cluster(object):
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
             idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
             selector_node_states=self.selector_node_states, node_taints=self.node_taints,
-            pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity)
+            pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity,
+            anti_affinity_node_states=self.anti_affinity_node_states)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [

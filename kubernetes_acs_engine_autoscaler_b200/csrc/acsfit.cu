@@ -17,6 +17,7 @@
 #include <tuple>
 #include <vector>
 
+#include "acsfit_admit.cuh"
 #include "acsfit_kernels.cuh"
 #include "acsfit_rank.cuh"
 #include "acsfit_stream.cuh"
@@ -2194,6 +2195,61 @@ extern "C" acsfit_status acsfit_node_states(acsfit_ctx *ctx, const int64_t *row_
     TRY(run_node_states(ctx, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age, N, D,
                         any_pending, thr_dev, S, out_state, st));
     CUDA_TRY(cudaStreamSynchronize(st));  // idle_threshold is a host buffer
+    return ACSFIT_OK;
+}
+
+static bool aligned8(const void *p) { return ((uintptr_t)p & 7u) == 0; }
+
+extern "C" acsfit_status acsfit_pending_admit(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
+                                              const uint64_t *run_matches, int64_t N, const uint64_t *node_match,
+                                              const uint8_t *sig_class, const uint64_t *sig_carries,
+                                              const uint64_t *sig_matches, int U, uint8_t *node_flags_inout,
+                                              acsfit_stream_t stream)
+{
+    TRY(enter(ctx, 1));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (N < 0 || U < 0 || (N > 0 && (!row_ptr || !node_flags_inout)) ||
+        (N > 0 && U > 0 && (!sig_class || !sig_carries || !sig_matches)))
+        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: bad arguments");
+    if (N == 0) return ACSFIT_OK;
+    if ((N + kAdmitBlock - 1) / kAdmitBlock > INT32_MAX)
+        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: N=%lld nodes is too many", (long long)N);
+    if (!aligned8(row_ptr) || !aligned8(run_carries) || !aligned8(run_matches) || !aligned8(node_match))
+        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: row_ptr and the mask arrays must be 8-byte aligned");
+    for (int u = 0; u < U; ++u)
+        if (sig_class[u] >= ACSFIT_MAX_CLASSES)
+            return fail(ctx, ACSFIT_E_INVALID, "pending_admit: signature %d has class %d, need < %d", u, sig_class[u],
+                        ACSFIT_MAX_CLASSES);
+    int64_t ends[2] = {0, 0};  // row_ptr[0], row_ptr[N]: the rows the kernel reads
+    CUDA_TRY(cudaMemcpyAsync(&ends[0], row_ptr, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&ends[1], row_ptr + N, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (ends[0] < 0 || ends[1] < ends[0])
+        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: row_ptr[0]=%lld, row_ptr[N]=%lld", (long long)ends[0],
+                    (long long)ends[1]);
+    if (ends[1] > ends[0] && (!run_carries || !run_matches))
+        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: %lld rows but a NULL run mask array",
+                    (long long)(ends[1] - ends[0]));
+    const size_t Uq = (size_t)std::max(U, 1);
+    TRY(arena_reserve(ctx, Uq * (2 * sizeof(uint64_t) + 1) + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(d_carries, unsigned long long, Uq);
+    TAKE(d_matches, unsigned long long, Uq);
+    TAKE(d_class, uint8_t, Uq);
+    if (U > 0) {
+        CUDA_TRY(cudaMemcpyAsync(d_carries, sig_carries, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_matches, sig_matches, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_class, sig_class, U, cudaMemcpyHostToDevice, st));
+    }
+    const int grid = (int)((N + kAdmitBlock - 1) / kAdmitBlock);
+    pending_admit_kernel<<<grid, kAdmitBlock, 0, st>>>(
+        row_ptr, reinterpret_cast<const unsigned long long *>(run_carries),
+        reinterpret_cast<const unsigned long long *>(run_matches), N,
+        reinterpret_cast<const unsigned long long *>(node_match), d_class, d_carries, d_matches, U, node_flags_inout);
+    ctx->scan_rec = {3, kScanPerThread, 0, kAdmitSmem, kAdmitBlock / 32, kAdmitBlock, grid, U};
+    ++ctx->launches;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));  // the signature table is a host buffer
     return ACSFIT_OK;
 }
 

@@ -254,6 +254,22 @@ class Engine(object):
                                                  _ptr(out), self._stream()))
         return out
 
+    def pending_admit(self, row_ptr, run_carries, run_matches, node_match, sig_class, sig_carries, sig_matches,
+                      node_flags):
+        """set ACSFIT_NODEF_NO_PENDING_MATCH on the nodes no signature (class, carries, matches) admits (include/acsfit.h,
+        acsfit_pending_admit).  row_ptr int64 [N+1], run_carries / run_matches uint64 [rows] (stored as int64),
+        node_match uint64 [N] or None, node_flags uint8 [N]: device, node_flags updated in place.  The signature
+        arrays are host arrays of one length U."""
+        N = node_flags.shape[0]
+        sig_class = _np(sig_class, np.uint8)
+        sig_carries, sig_matches = _np(sig_carries, np.uint64), _np(sig_matches, np.uint64)
+        U = sig_class.shape[0]
+        assert sig_carries.shape == sig_matches.shape == (U,)
+        self._check(self._lib.acsfit_pending_admit(self._ctx, _ptr(row_ptr), _ptr(run_carries), _ptr(run_matches), N,
+                                                   _ptr(node_match), _ptr(sig_class), _ptr(sig_carries),
+                                                   _ptr(sig_matches), U, _ptr(node_flags), self._stream()))
+        return node_flags
+
     def maintain_actions(self, state, node_pool, budget0, pool_scalable, dry_run):
         """engine_scaler.py:133-182 decisions. `state` uint8[N] device is rewritten; returns action uint8[N]."""
         N = state.shape[0]

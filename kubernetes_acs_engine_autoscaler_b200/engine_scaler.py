@@ -22,7 +22,8 @@ ACT_NONE, ACT_CORDON_DRAIN, ACT_CORDON, ACT_UNCORDON, ACT_SCALE_IN = range(5)
 class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                  deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
-                 selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False):
+                 selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False,
+                 anti_affinity_node_states=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
@@ -30,6 +31,7 @@ class EngineScaler(Scaler):
         self.node_taints = node_taints
         self.node_affinity = node_affinity
         self.pod_anti_affinity = pod_anti_affinity
+        self.anti_affinity_node_states = anti_affinity_node_states
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)
@@ -116,7 +118,8 @@ class EngineScaler(Scaler):
         if nodes:
             lists = [pods_by_node.get(node.name, []) for node in nodes]
             state_dev = snapshot.node_states(nodes, lists, bool(pods_to_schedule), self.idle_threshold,
-                                             no_match=self.no_pending_match(nodes, pods_to_schedule))
+                                             **self.pending_flags(nodes, lists, pods_to_schedule,
+                                                                  running_or_pending_assigned_pods))
             states, actions = snapshot.maintain_actions(state_dev, node_pool, budget0, [1] * len(budget0),
                                                         self.dry_run)
             info = logger.isEnabledFor(logging.INFO)  # (formatted eagerly, as upstream: skipped when nobody listens)

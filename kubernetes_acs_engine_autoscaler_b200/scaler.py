@@ -72,6 +72,9 @@ class Scaler(object):
         self.node_affinity = False
         # required pod anti-affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_anti_affinity=...))
         self.pod_anti_affinity = False
+        # with pod anti-affinity: POD_PENDING only when some pod to schedule could land on the node given the pods
+        # already there (Cluster(anti_affinity_node_states=...))
+        self.anti_affinity_node_states = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -86,11 +89,26 @@ class Scaler(object):
             return None
         return ~snapshot.pending_match(pods_to_schedule, nodes, taints=self.node_taints, affinity=self.node_affinity)
 
+    def pending_flags(self, nodes, pods_lists, pods_to_schedule, running_pods):
+        """the keywords `no_match` and `admit` of snapshot.node_states.  With anti_affinity_node_states on, something
+        to schedule and some anti-affinity term that can block a pod to schedule, the GPU decides which nodes some pod
+        to schedule is admitted to (snapshot.pending_admit, node selectors included when selector_node_states is on);
+        otherwise no_pending_match decides."""
+        admit = None
+        if self.anti_affinity_node_states and pods_to_schedule:
+            admit = snapshot.pending_admit(pods_to_schedule, running_pods, nodes, pods_lists,
+                                           selectors=self.selector_node_states, taints=self.node_taints,
+                                           affinity=self.node_affinity)
+        if admit is not None:
+            return {"no_match": None, "admit": admit}
+        return {"no_match": self.no_pending_match(nodes, pods_to_schedule), "admit": None}
+
     def get_node_state(self, node, node_pods, pods_to_schedule):
         """ClusterNodeState of one node (scaler.py:61-114): a one-node launch of the idle scan.
         EngineScaler.maintain classifies all nodes in a single launch instead."""
-        code = snapshot.node_states([node], [list(node_pods)], bool(pods_to_schedule), self.idle_threshold,
-                                    no_match=self.no_pending_match([node], pods_to_schedule))
+        node_pods = list(node_pods)
+        code = snapshot.node_states([node], [node_pods], bool(pods_to_schedule), self.idle_threshold,
+                                    **self.pending_flags([node], [node_pods], pods_to_schedule, node_pods))
         return STATE_NAMES[int(code.cpu().numpy()[0])]
 
     def fulfill_pending(self, pods):

@@ -448,7 +448,36 @@ def anti_affinity(pods, nodes=(), running_pods=()):
     reads) projection of the pods, vectorised, not once per pod; nothing of size pods x terms is built."""
     pods, nodes = list(pods), list(nodes)
     row_ptr, run_idx = running_csr(nodes, running_pods) if nodes and running_pods else (None, np.zeros(0, np.int32))
+    carries, matches, row_carries, row_matches, terms = _anti_affinity_masks(pods, list(running_pods), run_idx)
+    node_carries = np.zeros(len(nodes), dtype=np.uint64)
+    node_matches = np.zeros(len(nodes), dtype=np.uint64)
+    if len(run_idx) and terms:
+        # OR over the running pods of each node
+        node_of = np.repeat(np.arange(len(nodes), dtype=np.int64), np.diff(row_ptr))
+        np.bitwise_or.at(node_carries, node_of, row_carries)
+        np.bitwise_or.at(node_matches, node_of, row_matches)
+    return AntiAffinity(carries, matches, node_carries, node_matches, terms)
+
+
+def anti_affinity_rows(pods, running_pods, pods_lists):
+    """anti_affinity's masks without the OR per node: (pod_carries uint64[P], pod_matches uint64[P], row_carries uint64[R],
+    row_matches uint64[R], terms), with one row per entry of the concatenated `pods_lists` (node_states' table).  Every
+    pod of `pods_lists` is an object of `running_pods`, grouped per node as the occupancy count groups them; the terms,
+    their numbering and their dropping are then those of anti_affinity(pods, nodes, running_pods).  Raises ValueError
+    for a pod of `pods_lists` that is not in `running_pods`."""
     running = list(running_pods)
+    ids = np.fromiter(map(id, running), dtype=np.int64, count=len(running))
+    order = np.argsort(ids, kind="stable")
+    flat = np.fromiter(map(id, itertools.chain.from_iterable(pods_lists)), dtype=np.int64)
+    pos = np.searchsorted(ids[order], flat)
+    if len(flat) and ((pos >= len(ids)).any() or (ids[order[np.minimum(pos, len(ids) - 1)]] != flat).any()):
+        raise ValueError("a pod of pods_lists is not one of running_pods")
+    return _anti_affinity_masks(list(pods), running, order[pos] if len(flat) else np.zeros(0, np.int64))
+
+
+def _anti_affinity_masks(pods, running, run_idx):
+    """(pod_carries[P], pod_matches[P], row_carries, row_matches, kept terms): the masks of the pods to place and of
+    running[run_idx[k]] for every k, for anti_affinity and anti_affinity_rows"""
     on_nodes = np.unique(run_idx)
     everyone = pods + [running[j] for j in on_nodes.tolist()]
     P = len(pods)
@@ -464,8 +493,8 @@ def anti_affinity(pods, nodes=(), running_pods=()):
             ids.append(k)
         carried.append(ids)
     if not terms:
-        return AntiAffinity(np.zeros(P, np.uint64), np.zeros(P, np.uint64), np.zeros(len(nodes), np.uint64),
-                            np.zeros(len(nodes), np.uint64), [])
+        return (np.zeros(P, np.uint64), np.zeros(P, np.uint64), np.zeros(len(run_idx), np.uint64),
+                np.zeros(len(run_idx), np.uint64), [])
     T = len(terms)
     keys = sorted({key for _, (items, reqs) in terms for key, *_ in items + reqs})
     group, proj, code_of = _pod_projection(everyone, keys)
@@ -504,15 +533,8 @@ def anti_affinity(pods, nodes=(), running_pods=()):
     carries = np.zeros(len(everyone), dtype=np.uint64)
     kept = bit_of[pair_term] >= 0
     np.bitwise_or.at(carries, pair_pod[kept], np.uint64(1) << bit_of[pair_term[kept]].astype(np.uint64))
-    node_carries = np.zeros(len(nodes), dtype=np.uint64)
-    node_matches = np.zeros(len(nodes), dtype=np.uint64)
-    if len(run_idx):
-        # OR over the running pods of each node (a pod is in `everyone` at P + its rank in on_nodes)
-        at = P + np.searchsorted(on_nodes, run_idx)
-        node_of = np.repeat(np.arange(len(nodes), dtype=np.int64), np.diff(row_ptr))
-        np.bitwise_or.at(node_carries, node_of, carries[at])
-        np.bitwise_or.at(node_matches, node_of, matches[at])
-    return AntiAffinity(carries[:P], matches[:P], node_carries, node_matches, [terms[k] for k in keep.tolist()])
+    at = P + np.searchsorted(on_nodes, run_idx)  # a running pod is in `everyone` at P + its rank in on_nodes
+    return carries[:P], matches[:P], carries[at], matches[at], [terms[k] for k in keep.tolist()]
 
 
 # ------------------------------------------------------------------------------------------------
@@ -744,10 +766,45 @@ def node_age_seconds(node, now_by_tz=None):
     return (now - node.creation_time).seconds
 
 
-def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None):
+class PendingAdmit(object):
+    """what acsfit_pending_admit reads beside node_states' table: row_carries / row_matches uint64[R] (one per row of the
+    table), node_match uint64[N] class masks or None (every pod matches every node), and the U distinct signatures
+    (class, carries, matches) of the pods to schedule: sig_class uint8[U], sig_carries / sig_matches uint64[U]."""
+
+    def __init__(self, row_carries, row_matches, node_match, sig_class, sig_carries, sig_matches):
+        self.row_carries = row_carries
+        self.row_matches = row_matches
+        self.node_match = node_match
+        self.sig_class = sig_class
+        self.sig_carries = sig_carries
+        self.sig_matches = sig_matches
+
+
+def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints=False, affinity=False):
+    """the PendingAdmit of node_states(admit=...): node n stays pod-pending only when some pod of `pods` (the pods to
+    schedule) is blocked by no pod of pods_lists[n] (the node's pods, objects of `running_pods`) in either direction,
+    and, with `selectors`, matches the node as pending_match(pods, nodes, taints, affinity) decides.  The masks are
+    anti_affinity_rows'; the classes selector_classes(pods, nodes, [], taints, affinity)'s (ValueError above 64).
+    None when no term is kept: nothing can block a pod to schedule, and pending_match alone decides."""
+    pods = list(pods)
+    pod_carries, pod_matches, row_carries, row_matches, terms = anti_affinity_rows(pods, running_pods, pods_lists)
+    if not terms:
+        return None
+    pod_class, node_match = np.zeros(len(pods), dtype=np.uint8), None
+    if selectors:
+        classes = selector_classes(pods, nodes, [], taints=taints, affinity=affinity)
+        if not classes.trivial:
+            pod_class, node_match = classes.pod_class, classes.node_match
+    sig = np.unique(np.stack([pod_class.astype(np.uint64), pod_carries, pod_matches], axis=1), axis=0)
+    return PendingAdmit(row_carries, row_matches, node_match, sig[:, 0].astype(np.uint8),
+                        np.ascontiguousarray(sig[:, 1]), np.ascontiguousarray(sig[:, 2]))
+
+
+def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None, admit=None):
     """state code per node (include/acsfit.h ACSFIT_ST_*); pods_lists[n] = the node's pods in order.  `no_match`
     (bool[N], optional): nodes no pod to schedule matches (~pending_match); they are classified as if there were no
-    pod to schedule (ACSFIT_NODEF_NO_PENDING_MATCH)."""
+    pod to schedule (ACSFIT_NODEF_NO_PENDING_MATCH).  `admit` (pending_admit(..., pods_lists=pods_lists), optional):
+    the same flag for the nodes that no pod to schedule is admitted to, set on the GPU (acsfit_pending_admit)."""
     nodes = list(nodes)
     if not nodes:
         return np.zeros(0, dtype=np.uint8)
@@ -767,11 +824,19 @@ def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None):
         node_flags |= np.where(np.asarray(no_match, dtype=bool), np.uint8(NODE_NO_PENDING_MATCH), np.uint8(0))
     age = np.asarray([node_age_seconds(n, clock) for n in nodes], dtype=np.int64)
     eng = get_engine()
-    st = eng.node_states(eng.dev(row_ptr, torch.int64),
+    d_row_ptr, d_node_flags = eng.dev(row_ptr, torch.int64), eng.dev(node_flags, torch.uint8)
+    if admit is not None:
+        if len(admit.row_carries) != len(flat):
+            raise ValueError("pending_admit masks of %d pods for a table of %d" % (len(admit.row_carries), len(flat)))
+        eng.pending_admit(d_row_ptr, eng.dev(admit.row_carries.view(np.int64), torch.int64),
+                          eng.dev(admit.row_matches.view(np.int64), torch.int64),
+                          None if admit.node_match is None else eng.dev(admit.node_match.view(np.int64), torch.int64),
+                          admit.sig_class, admit.sig_carries, admit.sig_matches, d_node_flags)
+    st = eng.node_states(d_row_ptr,
                          None,  # contiguous table: the rows ARE in node order (bulk-copy streaming kernel)
                          eng.dev(req_run, torch.float64), eng.dev(flags, torch.uint8),
                          eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32),
-                         eng.dev(node_flags, torch.uint8), eng.dev(age, torch.int64), any_pending,
+                         d_node_flags, eng.dev(age, torch.int64), any_pending,
                          np.asarray([idle_threshold], dtype=np.int64))
     return st[0].contiguous()
 
