@@ -417,6 +417,63 @@ ACSFIT_API acsfit_status acsfit_fulfill_pending_aa(acsfit_ctx *ctx, const double
                                                    int32_t *out_bin_of, int64_t *out_unaccounted,
                                                    uint64_t *out_evals, acsfit_stream_t stream);
 
+/*
+ * Required pod affinity (opt-in): spec.affinity.podAffinity.requiredDuringSchedulingIgnoredDuringExecution terms with
+ * topologyKey kubernetes.io/hostname.  A pod's signature is the set of its honoured terms; the host numbers the
+ * distinct signatures of the pods to place (at most ACSFIT_MAX_PA_SIGNATURES), bit s = signature s.  A pod matches a
+ * signature when every term of it selects the pod.  Per pod: pod_requires = its signature's bit (0: no constraint),
+ * pod_matches = the signatures it matches, pod_self = pod_requires & pod_matches.  Per node: node_has = the OR of
+ * pod_matches over the pods on it, which the pass updates as it places pods; a new bin starts with 0.
+ *   rule          a pod with pod_requires != 0 may take a node (bin) only when (pod_requires & node_has) != 0, or
+ *                 (bootstrap) when no pod anywhere matches its signature at its turn and it matches it itself.
+ *                 "Anywhere": every node of the node pass, the signatures `present` names (fulfill: what the node pass
+ *                 left, typically the OR of node_has), and every bin opened so far in this call, pool after pool.
+ *                 The rule is one-way (placed pods' terms never constrain the incoming pod) and ANDs with resources,
+ *                 `sel` and `aa`
+ *   bin packing   a pod the rule keeps out of every bin, a new one included, opens no bin and is credited no bin
+ *                 test; the passes over fresh bins stop once a pass places no pod, and such pods stay unaccounted
+ *                 for the pool (they go on to the next pool)
+ *   counters      otherwise unchanged formulas (the affinity test is evaluated first and short-circuits)
+ *   exactness     the bootstrap exception depends on global order, so a pass runs with a flip position per
+ *                 signature absent at its start (+inf at first); a pod at position pos treats signature s as absent
+ *                 iff pos <= flip[s].  After a pass the earliest placement of a pod matching a still unfixed such
+ *                 signature fixes flip[s] there, and the pass (node pass: from its saved state; bins: the pool's whole
+ *                 packing) is run again.  Pods up to that position decide as before, so the result is the sequential
+ *                 scheduler's after at most 1 + (absent self-affine signatures that get placed) passes, and after one
+ *                 pass when no signature is absent (acsfit_last_affinity_reruns)
+ *   pod_requires, pod_self, pod_matches   [dev] one per row of req
+ *   node_has      [dev] N masks, read and written (node pass only; fulfill ignores it)
+ * acsfit_first_fit_nodes_pa / acsfit_fulfill_pending_pa take the arguments of the *_aa forms with `sel` and `aa` both
+ * allowed to be NULL, plus `pa` and (fulfill) `present`.  They run the anti-affinity form of the pipeline kernel with
+ * the affinity test added (zero anti-affinity masks when `aa` is NULL), barrier form only and unchained, and refuse
+ * with ACSFIT_E_INVALID: a NULL `pa` or mask array that is read, the checks of `sel` and `aa`, and cluster mode.
+ */
+#define ACSFIT_MAX_PA_SIGNATURES 64
+typedef struct acsfit_pod_affinity {
+    const uint64_t *pod_requires, *pod_self, *pod_matches;  /* [dev] one per row of req */
+    uint64_t *node_has;                                     /* [dev] N, in/out (node pass only) */
+} acsfit_pod_affinity;
+
+ACSFIT_API acsfit_status acsfit_first_fit_nodes_pa(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                   const int32_t *node_type, double *used_inout, int64_t N,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, int32_t *out_placed,
+                                                   uint64_t *out_decisions, acsfit_stream_t stream);
+ACSFIT_API acsfit_status acsfit_fulfill_pending_pa(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                   int64_t num_listed, int D, const double *unit,
+                                                   const int32_t *pool_actual, const int32_t *pool_max,
+                                                   const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, uint64_t present,
+                                                   int64_t *out_new_size, int64_t *out_units_needed,
+                                                   int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                                   int32_t *out_bin_of, int64_t *out_unaccounted,
+                                                   uint64_t *out_evals, acsfit_stream_t stream);
+/* test hook: passes the last *_pa call ran again (each fixes one flip) and those flips in order: out_flips[2k] =
+ * signature, out_flips[2k + 1] = position (fulfill: pending position; 2 * *out_reruns entries; may be NULL) */
+ACSFIT_API acsfit_status acsfit_last_affinity_reruns(const acsfit_ctx *ctx, int64_t *out_reruns, int64_t *out_flips);
+
 /* acsfit_occupancy_host = acsfit_occupancy with host buffers (reference cluster.py:165-168): R rows of req_run,
  * used_inout N x D is read, updated and written back. */
 ACSFIT_API acsfit_status acsfit_occupancy_host(acsfit_ctx *ctx, const int64_t *row_ptr, const int32_t *run_idx,

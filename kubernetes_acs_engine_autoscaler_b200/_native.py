@@ -65,6 +65,14 @@ SIGNATURES = {
                                           c_vp, c_vp, c_vp]),
     "acsfit_fulfill_pending_aa": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
                                           c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # pod affinity: the arguments of the _aa form (sel and aa may be NULL) plus a `const acsfit_pod_affinity *`
+    # (and, fulfill, the uint64 `present`)
+    "acsfit_first_fit_nodes_pa": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp, c_vp]),
+    "acsfit_fulfill_pending_pa": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
+                                          c_vp, c_vp, c_vp, ctypes.c_uint64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                          c_vp]),
+    "acsfit_last_affinity_reruns": (c_int, [c_vp, c_vp, c_vp]),
 }
 
 
@@ -77,6 +85,11 @@ class Selectors(ctypes.Structure):
 class AntiAffinity(ctypes.Structure):
     """struct acsfit_anti_affinity (include/acsfit.h)"""
     _fields_ = [("pod_carries", c_vp), ("pod_matches", c_vp), ("node_carries", c_vp), ("node_matches", c_vp)]
+
+
+class PodAffinity(ctypes.Structure):
+    """struct acsfit_pod_affinity (include/acsfit.h)"""
+    _fields_ = [("pod_requires", c_vp), ("pod_self", c_vp), ("pod_matches", c_vp), ("node_has", c_vp)]
 
 
 # one record of acsfit_last_launches (ACSFIT_LAUNCH_FIELDS ints), field names in order

@@ -55,7 +55,8 @@ class Cluster(object):
                  instance_init_time, resource_group, notifier, ignore_pools,
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
-                 node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None):
+                 node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None,
+                 pod_affinity=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -99,6 +100,13 @@ class Cluster(object):
         elif anti_affinity_node_states and not self.pod_anti_affinity:
             raise ValueError("anti_affinity_node_states=True needs pod_anti_affinity on")
         self.anti_affinity_node_states = bool(anti_affinity_node_states) and self.pod_anti_affinity
+        # honour required pod affinity with topologyKey kubernetes.io/hostname in first fit and bin packing, so that a pod
+        # which must sit beside another is neither simulated onto a node without one nor packed into a new node alone
+        # (opt-in; None: $ACSFIT_POD_AFFINITY).  Independent of node selectors and anti-affinity.
+        if pod_affinity is None:
+            pod_affinity = os.environ.get('ACSFIT_POD_AFFINITY', '0') not in ('', '0')
+        self.pod_affinity = bool(pod_affinity)
+        self.affinity_present = set()  # signatures the last node pass left on some node (scale() hands them on)
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -201,7 +209,7 @@ class Cluster(object):
             idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
             selector_node_states=self.selector_node_states, node_taints=self.node_taints,
             pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity,
-            anti_affinity_node_states=self.anti_affinity_node_states)
+            anti_affinity_node_states=self.anti_affinity_node_states, pod_affinity=self.pod_affinity)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [
@@ -231,7 +239,8 @@ class Cluster(object):
 
         With pod anti-affinity on, `running_pods` are the pods already on the nodes (the tick's running or assigned
         pending pods, which scale() passes): their terms block pods, and pods' terms block them.  Without it, only the
-        pods this call places count."""
+        pods this call places count.  With pod affinity on they are also what a pod's affinity can find on a node, and
+        the signatures the nodes hold afterwards are kept in self.affinity_present for the bin packing."""
         pods, nodes = list(pods), list(nodes)
         classes = None
         if self.node_selectors:
@@ -239,7 +248,12 @@ class Cluster(object):
         anti_affinity = None
         if self.pod_anti_affinity:
             anti_affinity = snapshot.anti_affinity(pods, nodes, running_pods or [])
-        placed = snapshot.first_fit_nodes(pods, nodes, classes=classes, anti_affinity=anti_affinity)
+        pod_affinity = None
+        if self.pod_affinity:
+            pod_affinity = snapshot.pod_affinity(pods, nodes, running_pods or [])
+        placed = snapshot.first_fit_nodes(pods, nodes, classes=classes, anti_affinity=anti_affinity,
+                                          pod_affinity=pod_affinity)
+        self.affinity_present = pod_affinity.present_signatures() if pod_affinity is not None else set()
         detail = len(pods) <= LOG_DETAIL_LIMIT
         pending_pods = []
         for i, pod in enumerate(pods):
@@ -260,7 +274,10 @@ class Cluster(object):
         logger.info("To schedule: {}".format(len(pods_to_schedule)))
         pending_pods = self.get_pending_pods(pods_to_schedule, nodes, running_pods=running_pods)
         if len(pending_pods) > 0:
-            scaler.fulfill_pending(pending_pods)
+            if self.pod_affinity:
+                scaler.fulfill_pending(pending_pods, affinity_present=self.affinity_present)
+            else:
+                scaler.fulfill_pending(pending_pods)
 
     def get_pods_to_schedule(self, pods, agent_pools):
         """pending, unassigned pods that fit an empty instance of at least one pool

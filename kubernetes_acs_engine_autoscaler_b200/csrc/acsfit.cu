@@ -54,6 +54,7 @@ struct acsfit_ctx {
     uint64_t last_sel_hits = 0;                         // hit entries of the selector node passes of the last call (acsfit_last_sel_hits)
     unsigned long long *retire_dev = nullptr;           // [2] dead warps / retired stages of the last call's bin passes
     bool retire_counted = false;                        // retire_dev was zeroed by a bin pass of the last call (acsfit_last_bin_retirement)
+    std::vector<int64_t> pa_flips;                      // (signature, position) fixed by the last *_pa call, one per rerun
     // launch records of the current API call (acsfit_last_launches); rec_* are set by the caller of a pipeline launch
     std::vector<std::array<int, ACSFIT_LAUNCH_FIELDS>> launch_log;
     int rec_chained = 0, rec_pool = -1;
@@ -374,6 +375,43 @@ __global__ void account_kernel(const int32_t *cur_bin, int64_t P, int32_t take, 
     }
     for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xFFFFFFFFu, c, o);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);
+}
+
+// pod affinity: out[0] |= the OR of v[idx ? idx[i] : i] over i < n with gate == nullptr or gate[i] >= 0
+__global__ void or_rows_kernel(const unsigned long long *v, const int32_t *idx, int64_t n, const int32_t *gate,
+                               unsigned long long *out)
+{
+    unsigned long long m = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        if (!gate || gate[i] >= 0) m |= v[idx ? idx[i] : i];
+    for (int o = 16; o > 0; o >>= 1) m |= __shfl_down_sync(0xFFFFFFFFu, m, o);
+    if ((threadIdx.x & 31) == 0 && m) atomicOr(out, m);
+}
+// flip position of each signature: a pod at position pos treats signature s as absent iff pos <= f[s]
+// (-1: present from the start, INT64_MAX: not placed yet)
+struct PaFlips {
+    long long f[64];
+};
+// pod affinity: the need of the pod at each position i < n (row idx ? idx[i] : i): its signature bit, or 0 while the
+// bootstrap exception lets it land anywhere (it matches its own signature, and the signature is absent at its turn)
+__global__ void pa_need_kernel(const unsigned long long *requires_, const unsigned long long *self, const int32_t *idx,
+                               int64_t n, const PaFlips fl, unsigned long long *need)
+{
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t row = idx ? idx[i] : i;
+        const unsigned long long r = requires_[row], sf = self[row];
+        need[i] = sf && i <= fl.f[__ffsll((long long)sf) - 1] ? 0ull : r;
+    }
+}
+// pod affinity: every pod_requires has at most one bit and pod_self is a subset of it; flag[0] |= 4 otherwise
+__global__ void pa_check_kernel(const unsigned long long *requires_, const unsigned long long *self, int64_t n, int *flag)
+{
+    int bad = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const unsigned long long r = requires_[i];
+        bad |= (r & (r - 1)) != 0 || (self[i] & ~r) != 0;
+    }
+    if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 4);
 }
 
 // domain check: requests must be >= 0 and not NaN; flag[0] |= 1 otherwise
@@ -958,6 +996,14 @@ extern "C" acsfit_status acsfit_last_bin_retirement(const acsfit_ctx *ctx, uint6
     return ACSFIT_OK;
 }
 
+extern "C" acsfit_status acsfit_last_affinity_reruns(const acsfit_ctx *ctx, int64_t *out_reruns, int64_t *out_flips)
+{
+    if (!ctx || !out_reruns) return ACSFIT_E_INVALID;
+    *out_reruns = (int64_t)ctx->pa_flips.size() / 2;
+    if (out_flips) std::copy(ctx->pa_flips.begin(), ctx->pa_flips.end(), out_flips);
+    return ACSFIT_OK;
+}
+
 extern "C" acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out)
 {
     static_assert(sizeof(ScanLaunch) == sizeof(int) * ACSFIT_SCAN_FIELDS, "one int per record field");
@@ -1161,22 +1207,22 @@ static acsfit_status launch_stream(acsfit_ctx *ctx, const PipelineParams &pp, in
 constexpr int kOneCtaSmemKb = 116;  // more than half of the 227 KB an SM offers: a second CTA cannot be resident
 // SEL: the node-selector form of a node pass, AA: the anti-affinity form of a node or bin pass (barrier form only:
 // both ignore the "stream" knob)
-template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false, bool AA = false>
+template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false, bool AA = false, bool PA = false>
 static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
     if constexpr (RW > 0 && D <= 8 && !PRUNE && !SEL && !AA) {
         if (stream_form_ok(ctx, D, RW, pp.Tn)) return launch_stream<D, BINS, RW>(ctx, pp, stages, st, resident);
     }
     constexpr int NT = stage_threads(D, BINS);
-    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL, AA>::bytes(pp.Tn);
+    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL, AA, PA>::bytes(pp.Tn);
     // D >= 8: ONE stage CTA per SM.  Whether two fit is an accident of the register allocation (the bins kernel has
     // been compiled to 128 and to 237 registers by neighbouring source revisions); at c3 a second CTA on the
     // frontier's SM costs the placement chain more than the extra resident stages give back.
     if (D >= 8) smem = std::max(smem, (size_t)kOneCtaSmemKb * 1024);
     if (ctx->smem_floor_kb > 0) smem = std::max(smem, (size_t)ctx->smem_floor_kb * 1024);  // occupancy knob
-    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL, AA>;
+    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL, AA, PA>;
     if (resident) {  // only asked: how many stages does the GPU hold at once?  (cached: the query costs ~10 us)
-        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0) | (AA ? 8 : 0), RW, pp.Tn);
+        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0) | (AA ? 8 : 0) | (PA ? 16 : 0), RW, pp.Tn);
         auto it = ctx->resident_cache.find(key);
         if (it == ctx->resident_cache.end()) {
             int per_sm = 0;
@@ -1191,7 +1237,7 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     PipelineParams q = pp;
     // more stages than the GPU holds at once: several waves, each streaming the whole pod list (see the kernel's publish)
     int held = 0;
-    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA>(ctx, pp, stages, st, &held)));
+    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA, PA>(ctx, pp, stages, st, &held)));
     q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
     q.retire = BINS && ctx->retire;
     if (BINS && RW > 0) {  // the first counted bin pass of a call zeroes the counters (in stream order before the later ones)
@@ -1214,39 +1260,41 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
 }
 
 // the instantiation is chosen by the rank layout of the call: 0 (float64 scan), 1, 2 or 4 packed words per row
-template <int D, bool BINS, bool PRUNE, bool SEL = false, bool AA = false>
+template <int D, bool BINS, bool PRUNE, bool SEL = false, bool AA = false, bool PA = false>
 static acsfit_status launch_pipeline_v(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
     switch (pp.rk.nw) {
-    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL, AA>(ctx, pp, stages, st, resident);
-    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL, AA>(ctx, pp, stages, st, resident);
-    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL, AA>(ctx, pp, stages, st, resident);
-    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL, AA>(ctx, pp, stages, st, resident);
+    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL, AA, PA>(ctx, pp, stages, st, resident);
+    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL, AA, PA>(ctx, pp, stages, st, resident);
+    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL, AA, PA>(ctx, pp, stages, st, resident);
+    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL, AA, PA>(ctx, pp, stages, st, resident);
     default: return fail(ctx, ACSFIT_E_INVALID, "rank layout with %d words", pp.rk.nw);
     }
 }
 
-// node pass with node selectors (pp.node_match != nullptr), AA: and anti-affinity masks: the same pruning rule as
-// below, barrier form only
-template <int D, bool AA = false>
+// node pass with node selectors (pp.node_match != nullptr), AA: and anti-affinity masks, PA: and pod-affinity masks:
+// the same pruning rule as below, barrier form only
+template <int D, bool AA = false, bool PA = false>
 static acsfit_status launch_pipeline_sel(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
     int prune = ctx->prune;
     if (prune < 0) {
         int resident = 0;
-        TRY((launch_pipeline_v<D, false, false, true, AA>(ctx, pp, stages, st, &resident)));
+        TRY((launch_pipeline_v<D, false, false, true, AA, PA>(ctx, pp, stages, st, &resident)));
         prune = stages > resident;
     }
-    if (prune) return launch_pipeline_v<D, false, true, true, AA>(ctx, pp, stages, st, nullptr);
-    return launch_pipeline_v<D, false, false, true, AA>(ctx, pp, stages, st, nullptr);
+    if (prune) return launch_pipeline_v<D, false, true, true, AA, PA>(ctx, pp, stages, st, nullptr);
+    return launch_pipeline_v<D, false, false, true, AA, PA>(ctx, pp, stages, st, nullptr);
 }
 
 template <int D, bool BINS>
 static acsfit_status launch_pipeline_t(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
     if constexpr (BINS) {
+        if (pp.pod_need) return launch_pipeline_v<D, true, false, false, true, true>(ctx, pp, stages, st, nullptr);
         if (pp.pod_carries) return launch_pipeline_v<D, true, false, false, true>(ctx, pp, stages, st, nullptr);
     } else {
+        if (pp.pod_need) return launch_pipeline_sel<D, true, true>(ctx, pp, stages, st);  // the entry point set node_match
         if (pp.pod_carries) return launch_pipeline_sel<D, true>(ctx, pp, stages, st);  // the entry point set node_match
         if (pp.node_match) return launch_pipeline_sel<D>(ctx, pp, stages, st);
         // Stage bounds + scan-list pruning (the PRUNE instantiation) pay when the pass is throughput-bound, i.e.
@@ -1680,6 +1728,7 @@ static void reset_stats(acsfit_ctx *ctx)
     ctx->last_stages = ctx->last_tiles = 0;
     ctx->last_sel_hits = 0;
     ctx->retire_counted = false;
+    ctx->pa_flips.clear();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1693,12 +1742,68 @@ static size_t first_fit_scratch(const acsfit_ctx *ctx, int64_t P, int64_t N)
 }
 
 // pod_class / node_match (device, both or neither): node selectors (the SEL form of the node pass; single GPU only)
+// pod affinity, before a pass: the needs of positions [0, n) under the flips and, when a signature is watched, the
+// first-placement slots reset to "not placed" (all ones)
+static acsfit_status pa_prepare(acsfit_ctx *ctx, const acsfit_pod_affinity *pa, const int32_t *idx, int64_t n,
+                                const PaFlips &fl, uint64_t watch, unsigned long long *need,
+                                unsigned long long *first_placed, cudaStream_t st)
+{
+    if (n > 0) {
+        pa_need_kernel<<<grid_for(ctx, n, 256), 256, 0, st>>>(reinterpret_cast<const unsigned long long *>(pa->pod_requires),
+                                                             reinterpret_cast<const unsigned long long *>(pa->pod_self),
+                                                             idx, n, fl, need);
+        ++ctx->launches;
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (watch) CUDA_TRY(cudaMemsetAsync(first_placed, 0xFF, sizeof(unsigned long long) * 64, st));
+    return ACSFIT_OK;
+}
+
+// pod affinity, after a pass that watched the still unfixed signatures of `watch`: fixes the flip of the one placed
+// earliest (the lowest signature on a tie) and sets `again`; leaves `again` false when none was placed
+static acsfit_status pa_next_flip(acsfit_ctx *ctx, const unsigned long long *first_placed, uint64_t watch,
+                                  uint64_t &fixed, PaFlips &fl, bool &again, cudaStream_t st)
+{
+    again = false;
+    const uint64_t open = watch & ~fixed;
+    if (!open) return ACSFIT_OK;
+    unsigned long long fp[64];
+    CUDA_TRY(cudaMemcpyAsync(fp, first_placed, sizeof fp, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    int best = -1;
+    for (int s = 0; s < 64; ++s)
+        if (((open >> s) & 1u) && fp[s] != ~0ull && (best < 0 || fp[s] < fp[best])) best = s;
+    if (best < 0) return ACSFIT_OK;
+    fl.f[best] = (long long)fp[best];
+    fixed |= 1ull << best;
+    ctx->pa_flips.push_back(best);
+    ctx->pa_flips.push_back((int64_t)fp[best]);
+    again = true;
+    return ACSFIT_OK;
+}
+
+// OR of v[idx ? idx[i] : i] over i < n (gate: only where gate[i] >= 0), to the host
+static acsfit_status or_rows(acsfit_ctx *ctx, const uint64_t *v, const int32_t *idx, int64_t n, const int32_t *gate,
+                             unsigned long long *scratch, uint64_t *out, cudaStream_t st)
+{
+    *out = 0;
+    if (n <= 0) return ACSFIT_OK;
+    CUDA_TRY(cudaMemsetAsync(scratch, 0, sizeof(unsigned long long), st));
+    or_rows_kernel<<<grid_for(ctx, n, 256), 256, 0, st>>>(reinterpret_cast<const unsigned long long *>(v), idx, n, gate,
+                                                         scratch);
+    ++ctx->launches;
+    CUDA_TRY(cudaMemcpyAsync(out, scratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return ACSFIT_OK;
+}
+
 // aa (needs pod_class / node_match): anti-affinity masks (the SEL + AA form; single GPU only)
+// pa (needs aa): pod-affinity masks (the SEL + AA + PA form), run again from the saved node state per fixed flip
 static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const int32_t *pod_idx, int64_t P, int D,
                                     const double *cap_type, const int32_t *node_type, double *used, int64_t N,
                                     int32_t *out_placed, unsigned long long *out_decisions, cudaStream_t st,
                                     const uint8_t *pod_class = nullptr, const unsigned long long *node_match = nullptr,
-                                    const acsfit_anti_affinity *aa = nullptr)
+                                    const acsfit_anti_affinity *aa = nullptr, const acsfit_pod_affinity *pa = nullptr)
 {
     if (ctx->world > 1)
         return cluster_first_fit(ctx, req, pod_idx, P, D, cap_type, node_type, used, N, out_placed, out_decisions, st);
@@ -1755,9 +1860,59 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
         CUDA_TRY(cudaMemsetAsync(hits, 0, sizeof(unsigned long long), st));
         pp.sel_hits = hits;
     }
+    // pod affinity: the signatures no node holds at the start that some pod of the list matches itself are watched;
+    // the pass runs again, from the saved node state, for every one that gets placed (include/acsfit.h)
+    PaFlips fl;
+    uint64_t watch = 0, fixed = 0;
+    double *used0 = nullptr;
+    unsigned long long *masks0 = nullptr, *need = nullptr;
+    if (pa) {
+        need = arena_take<unsigned long long>(ctx, P);
+        pp.pod_need = need;
+        pp.first_placed = arena_take<unsigned long long>(ctx, 64);
+        unsigned long long *red = arena_take<unsigned long long>(ctx, 1);
+        if (!need || !pp.first_placed || !red) return fail(ctx, ACSFIT_E_NOMEM, "scratch arena too small for pod affinity");
+        pp.pod_aff_matches = reinterpret_cast<const unsigned long long *>(pa->pod_matches);
+        pp.node_has = reinterpret_cast<unsigned long long *>(pa->node_has);
+        uint64_t present = 0, selfs = 0;
+        TRY(or_rows(ctx, pa->node_has, nullptr, N, nullptr, red, &present, st));
+        TRY(or_rows(ctx, pa->pod_self, pod_idx, P, nullptr, red, &selfs, st));
+        for (int s = 0; s < 64; ++s) fl.f[s] = ((present >> s) & 1u) ? -1 : INT64_MAX;
+        watch = selfs & ~present;
+        if (watch) {
+            used0 = arena_take<double>(ctx, (size_t)N * D);
+            masks0 = arena_take<unsigned long long>(ctx, (size_t)N * 3);
+            if (!used0 || !masks0) return fail(ctx, ACSFIT_E_NOMEM, "scratch arena too small for pod affinity");
+            CUDA_TRY(cudaMemcpyAsync(used0, used, sizeof(double) * N * D, cudaMemcpyDeviceToDevice, st));
+            CUDA_TRY(cudaMemcpyAsync(masks0, pp.node_has, sizeof(uint64_t) * N, cudaMemcpyDeviceToDevice, st));
+            CUDA_TRY(cudaMemcpyAsync(masks0 + N, pp.node_carries, sizeof(uint64_t) * N, cudaMemcpyDeviceToDevice, st));
+            CUDA_TRY(cudaMemcpyAsync(masks0 + 2 * N, pp.node_matches, sizeof(uint64_t) * N, cudaMemcpyDeviceToDevice, st));
+        }
+        pp.watch = watch;
+        TRY(pa_prepare(ctx, pa, pod_idx, P, fl, watch, need, pp.first_placed, st));
+    }
 
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
     TRY(launch_pipeline<false>(ctx, D, pp, plan.stages, st));
+    for (bool again = pa && watch;;) {
+        if (again) {
+            TRY(check_pipeline_status(ctx, status, st));
+            TRY(pa_next_flip(ctx, pp.first_placed, watch, fixed, fl, again, st));
+        }
+        if (!again) break;
+        // run the pass again from its start: node state, sync words, alive bits and placements
+        CUDA_TRY(cudaMemcpyAsync(used, used0, sizeof(double) * N * D, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(pp.node_has, masks0, sizeof(uint64_t) * N, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(pp.node_carries, masks0 + N, sizeof(uint64_t) * N, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(pp.node_matches, masks0 + 2 * N, sizeof(uint64_t) * N, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemsetAsync(sync_words, 0, sizeof(int) * (plan.stages + 8), st));
+        fill_alive_kernel<<<grid_for(ctx, alive_words, 256), 256, 0, st>>>(alive, P);
+        fill_i32_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(out_placed, P, -1);
+        ctx->launches += 2;
+        pp.watch = watch & ~fixed;
+        TRY(pa_prepare(ctx, pa, pod_idx, P, fl, pp.watch, need, pp.first_placed, st));
+        TRY(launch_pipeline<false>(ctx, D, pp, plan.stages, st));
+    }
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev1, st));
     if (out_decisions) {
         decisions_kernel<<<grid_for(ctx, P, 256), 256, 0, st>>>(out_placed, P, N, out_decisions);
@@ -1820,9 +1975,13 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                                   int32_t *out_acc_pool, int32_t *out_bin_of, int64_t *out_unaccounted,
                                   uint64_t *out_evals, cudaStream_t st, const FirstPassDone *pre = nullptr,
                                   const uint8_t *pod_class = nullptr, const uint64_t *pool_match_host = nullptr,
-                                  const acsfit_anti_affinity *aa = nullptr)
+                                  const acsfit_anti_affinity *aa = nullptr, const acsfit_pod_affinity *pa = nullptr,
+                                  uint64_t present = 0)
 {
     // aa: anti-affinity masks of the pods (indexed like req rows); every bin pass runs the AA form, unchained
+    // pa (needs aa): pod-affinity masks; every bin pass runs the AA + PA form.  `present`: the signatures already held
+    // (by the nodes); it gains those of the pods placed in each pool's bins.  A pool's packing runs again for every
+    // flip it fixes, and bin_of is written from the final run.
     // pod_class [dev] (indexed like req rows) + pool_match_host [host] T (visiting order): node selectors.  They only
     // change the pool gate: every bin of a pool carries the pool's labels, so the bin passes are the plain ones.
     for (int i = 0; i < T * D; ++i)
@@ -1842,6 +2001,18 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
     TAKE(evals_dev, unsigned long long, 1);
     TAKE(count_dev, unsigned long long, 1);
     TAKE(max_bin_dev, int, 1);
+    PaFlips fl;
+    uint64_t selfs = 0;
+    unsigned long long *need = nullptr, *first_placed = nullptr, *evals_save = nullptr;
+    if (pa) {
+        TAKE(need_, unsigned long long, Pp);
+        TAKE(fp_, unsigned long long, 64);
+        TAKE(red_, unsigned long long, 2);
+        need = need_;
+        first_placed = fp_;
+        evals_save = red_ + 1;
+        TRY(or_rows(ctx, pa->pod_self, row_map, Pp, nullptr, red_, &selfs, st));
+    }
 
     if (T > 0) CUDA_TRY(cudaMemcpyAsync(unit_dev, unit_host, sizeof(double) * T * D, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemsetAsync(evals_dev, 0, sizeof(unsigned long long), st));
@@ -1885,6 +2056,13 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
             CUDA_TRY(cudaMemsetAsync(max_bin_dev, 0xFF, sizeof(int), st));  // -1
             int32_t *list = list_a, *next = list_b;
             int64_t M = E, bin_base = 0;
+            uint64_t watch = 0, fixed = 0;
+            if (pa) {  // the signatures absent so far that some pod matches itself are watched
+                for (int s = 0; s < 64; ++s) fl.f[s] = ((present >> s) & 1u) ? -1 : INT64_MAX;
+                watch = selfs & ~present;
+                TRY(pa_prepare(ctx, pa, row_map, Pp, fl, watch, need, first_placed, st));
+                if (watch) CUDA_TRY(cudaMemcpyAsync(evals_save, evals_dev, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+            }
             if (first_done) {
                 CUDA_TRY(cudaMemcpyAsync(cur_bin, pre->cur_bin, sizeof(int32_t) * Pp, cudaMemcpyDeviceToDevice, st));
                 record_bins_kernel<<<grid_for(ctx, Pp, 256), 256, 0, st>>>(cur_bin, Pp, out_bin_of, max_bin_dev);
@@ -1960,13 +2138,19 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                     pp.pod_carries = reinterpret_cast<const unsigned long long *>(aa->pod_carries);
                     pp.pod_matches = reinterpret_cast<const unsigned long long *>(aa->pod_matches);
                 }
+                if (pa) {
+                    pp.pod_need = need;
+                    pp.pod_aff_matches = reinterpret_cast<const unsigned long long *>(pa->pod_matches);
+                    pp.first_placed = first_placed;
+                    pp.watch = watch & ~fixed;
+                }
                 if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
                 ctx->rec_pool = t;
                 TRY(launch_pipeline<true>(ctx, D, pp, plan.stages, st));
                 if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev1, st));
                 if (cl) TRY(cluster_merge_placed(ctx, M, placed, st));  // every rank: the pass's complete placements
-                scatter_bins_kernel<<<grid_for(ctx, M, 256), 256, 0, st>>>(list, placed, M, cur_bin, out_bin_of,
-                                                                          max_bin_dev);
+                scatter_bins_kernel<<<grid_for(ctx, M, 256), 256, 0, st>>>(list, placed, M, cur_bin,
+                                                                          pa ? cur_bin : out_bin_of, max_bin_dev);
                 ++ctx->launches;
                 TRY(check_pipeline_status(ctx, pp.status, st));
                 if (ctx->timing) {
@@ -1984,7 +2168,33 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                 else TRY(compact(ctx, BitPred{alive}, M, list, next, block_counts, total_dev, &left, st));
                 bin_base += pass_bins;
                 std::swap(list, next);
+                // pod affinity: a pod may fit no bin, a fresh one included; once a pass places nothing the rest stays
+                // unaccounted for this pool.  When the packing is over and it placed a watched signature, it runs
+                // again from scratch with that signature's flip fixed.
+                if (pa && left == M) left = 0;
                 M = left;
+                if (pa && M == 0) {
+                    bool again = false;
+                    TRY(pa_next_flip(ctx, first_placed, watch, fixed, fl, again, st));
+                    if (again) {
+                        CUDA_TRY(cudaMemcpyAsync(evals_dev, evals_save, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+                        CUDA_TRY(cudaMemsetAsync(max_bin_dev, 0xFF, sizeof(int), st));
+                        fill_i32_kernel<<<grid_for(ctx, Pp, 256), 256, 0, st>>>(cur_bin, Pp, -1);
+                        ++ctx->launches;
+                        list = list_a;
+                        next = list_b;
+                        TRY(compact(ctx, FlagPred{elig}, Pp, nullptr, list, block_counts, total_dev, &M, st));
+                        bin_base = 0;
+                        TRY(pa_prepare(ctx, pa, row_map, Pp, fl, watch & ~fixed, need, first_placed, st));
+                    }
+                }
+            }
+            if (pa) {  // bin_of from the final run; the signatures of the pods it placed are present from now on
+                record_bins_kernel<<<grid_for(ctx, Pp, 256), 256, 0, st>>>(cur_bin, Pp, out_bin_of, max_bin_dev);
+                ++ctx->launches;
+                uint64_t placed_sigs = 0;
+                TRY(or_rows(ctx, pa->pod_matches, row_map, Pp, cur_bin, first_placed, &placed_sigs, st));
+                present |= placed_sigs;
             }
             int max_bin = -1;
             CUDA_TRY(cudaMemcpyAsync(&max_bin, max_bin_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2846,34 +3056,76 @@ static acsfit_status check_aa_host(acsfit_ctx *ctx, const acsfit_anti_affinity *
     return ACSFIT_OK;
 }
 
-extern "C" acsfit_status acsfit_first_fit_nodes_aa(acsfit_ctx *ctx, const double *req, int64_t req_rows,
-                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
-                                                   const int32_t *node_type, double *used_inout, int64_t N,
-                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
-                                                   int32_t *out_placed, uint64_t *out_decisions,
-                                                   acsfit_stream_t stream)
+// pod affinity (include/acsfit.h, acsfit_pod_affinity): the *_pa entry points share the *_aa ones' implementation
+static acsfit_status check_pa_host(acsfit_ctx *ctx, const acsfit_pod_affinity *pa, int64_t rows, int64_t N,
+                                   int *flag_dev, cudaStream_t st, const char *what)
+{
+    if (!pa) return fail(ctx, ACSFIT_E_INVALID, "%s: pod-affinity masks missing", what);
+    if (ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: pod affinity is not supported in cluster mode", what);
+    if ((rows > 0 && (!pa->pod_requires || !pa->pod_self || !pa->pod_matches)) || (N > 0 && !pa->node_has))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: pod-affinity field missing", what);
+    if (rows <= 0) return ACSFIT_OK;
+    CUDA_TRY(cudaMemsetAsync(flag_dev, 0, sizeof(int), st));
+    pa_check_kernel<<<grid_for(ctx, rows, 256), 256, 0, st>>>(reinterpret_cast<const unsigned long long *>(pa->pod_requires),
+                                                              reinterpret_cast<const unsigned long long *>(pa->pod_self),
+                                                              rows, flag_dev);
+    ++ctx->launches;
+    int flag = 0;
+    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    if (flag & 4) return fail(ctx, ACSFIT_E_INVALID, "%s: a pod_requires has more than one bit, or pod_self is not inside it", what);
+    return ACSFIT_OK;
+}
+
+// zero anti-affinity masks for a pod-affinity call without `aa` (rows pods, N nodes), from the arena
+static acsfit_status zero_aa(acsfit_ctx *ctx, int64_t rows, int64_t N, acsfit_anti_affinity *out, cudaStream_t st)
+{
+    TAKE(z, uint64_t, (size_t)2 * rows + (size_t)2 * N);
+    CUDA_TRY(cudaMemsetAsync(z, 0, sizeof(uint64_t) * std::max<size_t>(1, (size_t)2 * rows + (size_t)2 * N), st));
+    *out = {z, z + rows, z + 2 * rows, z + 2 * rows + N};
+    return ACSFIT_OK;
+}
+
+// pa == nullptr: the *_aa form (aa required); otherwise the *_pa form (aa may be NULL)
+static acsfit_status first_fit_nodes_aa_pa(acsfit_ctx *ctx, const double *req, int64_t req_rows, const int32_t *pod_idx,
+                                           int64_t P, int D, const double *cap_type, const int32_t *node_type,
+                                           double *used_inout, int64_t N, const acsfit_selectors *sel,
+                                           const acsfit_anti_affinity *aa, const acsfit_pod_affinity *pa,
+                                           int32_t *out_placed, uint64_t *out_decisions, acsfit_stream_t stream,
+                                           const char *what)
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
         (P > 0 && (!req || !out_placed)) || (N > 0 && (!cap_type || !node_type || !used_inout)))
-        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_aa: bad arguments");
+        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
     if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_aa: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
-    TRY(check_req_aligned(ctx, req, "first_fit_nodes_aa"));
-    TRY(check_aa_host(ctx, aa, req_rows, N, "first_fit_nodes_aa"));
-    if (sel) TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, "first_fit_nodes_aa"));
+        return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
+    TRY(check_req_aligned(ctx, req, what));
+    if (!pa || aa) TRY(check_aa_host(ctx, aa, req_rows, N, what));
+    if (sel) TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, what));
     reset_stats(ctx);
     // without selectors: class 0 for every row and all-ones node masks, from the arena
     const size_t trivial = sel ? 0 : align_up((size_t)req_rows, 256) + sizeof(uint64_t) * (size_t)N + 512;
-    TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + trivial + 1024, st));
+    // pod affinity: zero anti-affinity masks without `aa`, the needs, and the saved node state of a rerun
+    const size_t pa_bytes = !pa ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)(req_rows + N) + 256) +
+                                          sizeof(uint64_t) * (size_t)P + sizeof(double) * (size_t)N * D +
+                                          sizeof(uint64_t) * 3 * (size_t)N + 2048;
+    TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + trivial + pa_bytes + 1024, st));
     ctx->arena_off = 0;
     TAKE(flag, int, 1);
     TRY(check_domain(ctx, req, req_rows * D, flag, st, "req"));
+    if (pa) TRY(check_pa_host(ctx, pa, req_rows, N, flag, st, what));
+    acsfit_anti_affinity zero;
+    if (pa && !aa) {
+        TRY(zero_aa(ctx, req_rows, N, &zero, st));
+        aa = &zero;
+    }
     const uint8_t *pod_class;
     const unsigned long long *node_match;
     if (sel) {
-        TRY(check_classes(ctx, sel->pod_class, req_rows, sel->classes, flag, st, "first_fit_nodes_aa", sel->node_match, N));
+        TRY(check_classes(ctx, sel->pod_class, req_rows, sel->classes, flag, st, what, sel->node_match, N));
         pod_class = sel->pod_class;
         node_match = reinterpret_cast<const unsigned long long *>(sel->node_match);
     } else {
@@ -2886,7 +3138,72 @@ extern "C" acsfit_status acsfit_first_fit_nodes_aa(acsfit_ctx *ctx, const double
     }
     if (P > 0 && N > 0) TRY(build_ranks(ctx, req, req_rows, D, st));
     return first_fit_impl(ctx, req, pod_idx, P, D, cap_type, node_type, used_inout, N, out_placed,
-                          reinterpret_cast<unsigned long long *>(out_decisions), st, pod_class, node_match, aa);
+                          reinterpret_cast<unsigned long long *>(out_decisions), st, pod_class, node_match, aa, pa);
+}
+
+extern "C" acsfit_status acsfit_first_fit_nodes_aa(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                   const int32_t *node_type, double *used_inout, int64_t N,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   int32_t *out_placed, uint64_t *out_decisions,
+                                                   acsfit_stream_t stream)
+{
+    return first_fit_nodes_aa_pa(ctx, req, req_rows, pod_idx, P, D, cap_type, node_type, used_inout, N, sel, aa,
+                                 nullptr, out_placed, out_decisions, stream, "first_fit_nodes_aa");
+}
+
+extern "C" acsfit_status acsfit_first_fit_nodes_pa(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                   const int32_t *node_type, double *used_inout, int64_t N,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, int32_t *out_placed,
+                                                   uint64_t *out_decisions, acsfit_stream_t stream)
+{
+    if (ctx && !pa) return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_pa: pod-affinity masks missing");
+    return first_fit_nodes_aa_pa(ctx, req, req_rows, pod_idx, P, D, cap_type, node_type, used_inout, N, sel, aa, pa,
+                                 out_placed, out_decisions, stream, "first_fit_nodes_pa");
+}
+
+static acsfit_status fulfill_pending_aa_pa(acsfit_ctx *ctx, const double *req, int64_t Pp, int64_t num_listed, int D,
+                                           const double *unit, const int32_t *pool_actual, const int32_t *pool_max,
+                                           const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                           const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                           const acsfit_pod_affinity *pa, uint64_t present, int64_t *out_new_size,
+                                           int64_t *out_units_needed, int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                           int32_t *out_bin_of, int64_t *out_unaccounted, uint64_t *out_evals,
+                                           acsfit_stream_t stream, const char *what)
+{
+    TRY(enter(ctx, D));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
+        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
+        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
+                   !out_bins_opened)) ||
+        !out_unaccounted)
+        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
+    TRY(check_req_aligned(ctx, req, what));
+    if (!pa || aa) TRY(check_aa_host(ctx, aa, Pp, 0, what));
+    if (sel) TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, what));
+    reset_stats(ctx);
+    const size_t pa_bytes = !pa ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)Pp + 256) + sizeof(uint64_t) * (size_t)Pp + 2048;
+    TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + pa_bytes + 1024, st));
+    ctx->arena_off = 0;
+    TAKE(flag, int, 1);
+    TRY(check_domain(ctx, req, Pp * D, flag, st, "req"));
+    if (pa) TRY(check_pa_host(ctx, pa, Pp, 0, flag, st, what));
+    acsfit_anti_affinity zero;
+    if (pa && !aa) {
+        TRY(zero_aa(ctx, Pp, 0, &zero, st));
+        aa = &zero;
+    }
+    if (sel) TRY(check_classes(ctx, sel->pod_class, Pp, sel->classes, flag, st, what));
+    TRY(build_ranks(ctx, req, Pp, D, st));
+    return fulfill_impl(ctx, req, nullptr, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                        over_provision, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
+                        out_unaccounted, out_evals, st, nullptr, sel ? sel->pod_class : nullptr,
+                        sel ? sel->pool_match_ordered : nullptr, aa, pa, present);
 }
 
 extern "C" acsfit_status acsfit_fulfill_pending_aa(acsfit_ctx *ctx, const double *req, int64_t Pp,
@@ -2899,30 +3216,26 @@ extern "C" acsfit_status acsfit_fulfill_pending_aa(acsfit_ctx *ctx, const double
                                                    int32_t *out_bin_of, int64_t *out_unaccounted,
                                                    uint64_t *out_evals, acsfit_stream_t stream)
 {
-    TRY(enter(ctx, D));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
-        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
-        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
-                   !out_bins_opened)) ||
-        !out_unaccounted)
-        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_aa: bad arguments");
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_aa: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
-    TRY(check_req_aligned(ctx, req, "fulfill_pending_aa"));
-    TRY(check_aa_host(ctx, aa, Pp, 0, "fulfill_pending_aa"));
-    if (sel) TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, "fulfill_pending_aa"));
-    reset_stats(ctx);
-    TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + 1024, st));
-    ctx->arena_off = 0;
-    TAKE(flag, int, 1);
-    TRY(check_domain(ctx, req, Pp * D, flag, st, "req"));
-    if (sel) TRY(check_classes(ctx, sel->pod_class, Pp, sel->classes, flag, st, "fulfill_pending_aa"));
-    TRY(build_ranks(ctx, req, Pp, D, st));
-    return fulfill_impl(ctx, req, nullptr, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
-                        over_provision, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
-                        out_unaccounted, out_evals, st, nullptr, sel ? sel->pod_class : nullptr,
-                        sel ? sel->pool_match_ordered : nullptr, aa);
+    return fulfill_pending_aa_pa(ctx, req, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                                 over_provision, sel, aa, nullptr, 0, out_new_size, out_units_needed, out_bins_opened,
+                                 out_acc_pool, out_bin_of, out_unaccounted, out_evals, stream, "fulfill_pending_aa");
+}
+
+extern "C" acsfit_status acsfit_fulfill_pending_pa(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                   int64_t num_listed, int D, const double *unit,
+                                                   const int32_t *pool_actual, const int32_t *pool_max,
+                                                   const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, uint64_t present,
+                                                   int64_t *out_new_size, int64_t *out_units_needed,
+                                                   int64_t *out_bins_opened, int32_t *out_acc_pool,
+                                                   int32_t *out_bin_of, int64_t *out_unaccounted,
+                                                   uint64_t *out_evals, acsfit_stream_t stream)
+{
+    if (ctx && !pa) return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_pa: pod-affinity masks missing");
+    return fulfill_pending_aa_pa(ctx, req, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                                 over_provision, sel, aa, pa, present, out_new_size, out_units_needed, out_bins_opened,
+                                 out_acc_pool, out_bin_of, out_unaccounted, out_evals, stream, "fulfill_pending_pa");
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -160,6 +160,16 @@ struct PipelineParams {
     // bin passes with the packed-rank scan (appended; test hook acsfit_last_bin_retirement): [0] += warps whose bins
     // were all dead when their stage exited, [1] += stages whose warps were all dead.  nullptr: not counted
     unsigned long long *retire_count;
+    // required pod affinity (PA instantiations, built on the AA form; appended).  A pod may take a node (bin) only when
+    // its need is 0 or shares a bit with the node's node_has (the signatures the node's pods match); the taker ORs the
+    // pod's pod_aff_matches into node_has.  pod_need is the pod's signature bit with the bootstrap exception already
+    // applied (0 while the pod may land anywhere), indexed by position: list entry (node pass) or pending pod (bins).
+    // Node passes read and write node_has; bins start at 0 and are not written back.
+    const unsigned long long *pod_need;         // [positions]
+    const unsigned long long *pod_aff_matches;  // [req rows] signatures the pod matches
+    unsigned long long *node_has;               // [N] in/out (node pass)
+    unsigned long long *first_placed;           // [64]: atomicMin of the position of each placed pod that matches a watched signature
+    unsigned long long watch;                   // signatures whose first placement is recorded (0: none, nothing recorded)
 };
 
 __device__ __forceinline__ int ld_acquire(const int *p)
@@ -234,7 +244,7 @@ __device__ __forceinline__ void load_row(double (&r)[D], const double *src)
 // dynamic shared memory layout (doubles first for alignment).
 // nodes mode keeps three [D][Tn] arrays: scan thresholds, used (the mutable state) and capacity;
 // bins mode keeps one: the remaining capacity IS the threshold (finite values, Lemma B).
-template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false, bool AA = false>
+template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false, bool AA = false, bool PA = false>
 struct PipelineSmem {
     static constexpr int NW = NT / 32;  // warps per stage CTA == resolver warps
     static __host__ __device__ size_t bytes(int Tn)
@@ -247,6 +257,7 @@ struct PipelineSmem {
                + sizeof(unsigned) * ((size_t)RW * Tn /*packed node words*/ + (size_t)RW * kTile /*packed pod words*/ + 4 /*alignment*/)
                + (SEL ? sizeof(unsigned long long) * (size_t)Tn /*node masks*/ + kTile /*pod classes*/ + (size_t)NW * 36 /*batch classes*/ : 0)
                + (AA ? sizeof(unsigned long long) * 2 * ((size_t)Tn /*node carries / matches*/ + kTile /*pod masks*/ + (size_t)NW * 36 /*batch masks*/) : 0)
+               + (PA ? sizeof(unsigned long long) * ((size_t)Tn /*node has*/ + 2 * ((size_t)kTile /*pod need / matches*/ + (size_t)NW * 36 /*batch*/)) : 0)
                + (BINS && RW > 0 ? sizeof(double) * (size_t)D * (1 /*smallest request*/ + kRankStaged /*staged rank tables*/) : 0);
     }
 };
@@ -293,12 +304,20 @@ __device__ __forceinline__ unsigned wait_entry(const volatile unsigned *slot, in
 // bits, so a pod blocked under older state is blocked now too: the resource-only (plus class) scan, the stale
 // thresholds, the bounds, pruning and the untouched-bin shortcut (a new bin has both masks 0 and blocks nobody) all
 // stay exact.  AA runs the barrier form only.
-template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false, bool AA = false>
+//
+// PA (on top of the AA form): required pod affinity.  A pod whose need is non-zero may take a node (bin) only when the
+// node's has mask shares a bit with it; the taker ORs the pod's signature matches into the node's mask.  A node's mask
+// only gains bits, so the test is NOT monotone the way the block test is: it is left out of the scan and the bounds,
+// which stay resource (plus class) only and hence a superset filter, and is evaluated in the resolver alone, whose
+// chain sees every node's state exactly as the sequential loop does.  The need itself is fixed for the pass (the host
+// applies the bootstrap exception through flip positions, see acsfit.cu).
+template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false, bool AA = false, bool PA = false>
 __global__ void __launch_bounds__(NT, D <= 4 ? 2 : 1)
 firstfit_pipeline_kernel(const PipelineParams p)
 {
     static_assert(!(SEL && BINS), "selectors apply to node passes only");
     static_assert(!AA || BINS || SEL, "the anti-affinity node pass builds on the selector form");
+    static_assert(!PA || AA, "the pod-affinity form builds on the anti-affinity form");
     constexpr int K = nodes_per_thread(D, RW);  // RW: 32-bit words of a packed-rank row, 0 = float64 scan
     constexpr int NW = NT / 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -339,8 +358,14 @@ firstfit_pipeline_kernel(const PipelineParams p)
     unsigned long long *px_s = pc_s + kTile;                                                            // [kTile]
     unsigned long long *bc_s = px_s + kTile;                                                            // [NW][36]
     unsigned long long *bx_s = bc_s + NW * 36;                                                          // [NW][36]
+    // PA: has masks of the stage's nodes, need / matches of the tile's compacted pods and of each resolver batch
+    unsigned long long *nh_s = AA ? bx_s + NW * 36 : nm_s;  // [Tn]
+    unsigned long long *pn_s = nh_s + Tn;                   // [kTile]
+    unsigned long long *pm_s = pn_s + kTile;                // [kTile]
+    unsigned long long *bn_s = pm_s + kTile;                // [NW][36]
+    unsigned long long *bm_s = bn_s + NW * 36;              // [NW][36]
     // bins with the packed-rank scan: the smallest request of each dimension and the staged rank tables
-    double *minreq_s = reinterpret_cast<double *>(AA ? bx_s + NW * 36 : nm_s);  // [D]
+    double *minreq_s = reinterpret_cast<double *>(PA ? bm_s + NW * 36 : AA ? bx_s + NW * 36 : nm_s);  // [D]
     double *rt_s = minreq_s + D;                                                 // [D][kRankStaged]
 
     const int tid = threadIdx.x;
@@ -404,6 +429,8 @@ firstfit_pipeline_kernel(const PipelineParams p)
             nc_s[n] = !BINS && n < n_valid ? p.node_carries[stage_lo + n] : 0ull;
             nx_s[n] = !BINS && n < n_valid ? p.node_matches[stage_lo + n] : 0ull;
         }
+    if constexpr (PA)
+        for (int n = tid; n < Tn; n += NT) nh_s[n] = !BINS && n < n_valid ? p.node_has[stage_lo + n] : 0ull;
     // Bin retirement (RW > 0).  The rank tables are built over every request row of the call, a superset of the pass's
     // pods, so sorted[d][0] is a lower bound of every request of the pass in dimension d.  A bin with S[d] < that
     // bound in some d can take no pod of the pass now, and S only shrinks: it is dead for good.  Without rank tables
@@ -485,6 +512,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
     unsigned prew[RW > 0 ? RW : 1];
     unsigned pre_cls = 0;  // SEL: the entry's selector class
     unsigned long long pre_c = 0ull, pre_x = 0ull;  // AA: the entry's carries / matches
+    unsigned long long pre_n = 0ull, pre_m = 0ull;  // PA: the entry's need / signature matches
     auto prefetch_row = [&](int tile) {
         const int64_t j = (int64_t)(p.tile_lo + tile) * kTile + tid;
         if (tid < kTile && tile < p.num_tiles && j < p.M) {
@@ -505,6 +533,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
             if constexpr (AA) {
                 pre_c = __ldg(p.pod_carries + row);
                 pre_x = __ldg(p.pod_matches + row);
+            }
+            if constexpr (PA) {
+                pre_n = __ldg(p.pod_need + (BINS ? (int64_t)__ldg(p.pod_idx + j) : j));
+                pre_m = __ldg(p.pod_aff_matches + row);
             }
         }
     };
@@ -627,6 +659,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
             if constexpr (AA) {
                 pc_s[pos] = pre_c;
                 px_s[pos] = pre_x;
+            }
+            if constexpr (PA) {
+                pn_s[pos] = pre_n;
+                pm_s[pos] = pre_m;
             }
         }
         prefetch_row(tile + 1);
@@ -853,6 +889,8 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     my_nc = n < Tn ? nc_s[n] : 0ull;
                     my_nx = n < Tn ? nx_s[n] : 0ull;
                 }
+                unsigned long long my_nh = 0ull;  // PA: this lane's node's has mask
+                if constexpr (PA) my_nh = n < Tn ? nh_s[n] : 0ull;
 
                 unsigned my_takes = 0;  // pods this lane's node / bin took in this tile
                 const volatile unsigned *in_q = BINS ? (chain_below ? queue + (size_t)(31 - __clz(chain_below)) * (kTile + 1) : hitlist)
@@ -932,6 +970,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     const int my_rank = __popc(possmask & ((1u << lane) - 1u));
                     unsigned char *bcls = bcls_s + warp * 36;  // SEL: class of each dense entry (+4 padding entries)
                     unsigned long long *bc = bc_s + warp * 36, *bx = bx_s + warp * 36;  // AA: masks of each dense entry
+                    unsigned long long *bn = bn_s + warp * 36, *bm = bm_s + warp * 36;  // PA: need / matches of each dense entry
                     if (poss) {
 #pragma unroll
                         for (int d = 0; d < D; d += 2)
@@ -940,6 +979,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         if constexpr (AA) {
                             bc[my_rank] = pc_s[q_l];
                             bx[my_rank] = px_s[q_l];
+                        }
+                        if constexpr (PA) {
+                            bn[my_rank] = pn_s[q_l];
+                            bm[my_rank] = pm_s[q_l];
                         }
                     }
                     fnd[lane] = 0xFF;  // "nobody took dense entry `lane`" until a taker says otherwise
@@ -953,6 +996,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         if constexpr (AA) {
                             bc[n_poss + lane] = 0ull;
                             bx[n_poss + lane] = 0ull;
+                        }
+                        if constexpr (PA) {
+                            bn[n_poss + lane] = 0ull;
+                            bm[n_poss + lane] = 0ull;
                         }
                     }
                     __syncwarp();
@@ -968,6 +1015,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     if constexpr (AA) {
                         ec = bc[0];
                         ex = bx[0];
+                    }
+                    unsigned long long en = 0ull, em = 0ull;  // PA: the entry's need / matches, loaded one entry ahead
+                    if constexpr (PA) {
+                        en = bn[0];
+                        em = bm[0];
                     }
                     const long long t_l0 = tracing ? clock64() : 0;
                     if (tracing) n_iter += (unsigned)n_poss;
@@ -1005,9 +1057,15 @@ firstfit_pipeline_kernel(const PipelineParams p)
                             ec_next = bc[k + 1];
                             ex_next = bx[k + 1];
                         }
+                        unsigned long long en_next = 0ull, em_next = 0ull;
+                        if constexpr (PA) {
+                            en_next = bn[k + 1];
+                            em_next = bm[k + 1];
+                        }
                         bool ok = fits(S, r);
                         if constexpr (SEL) ok = ok & mt;
                         if constexpr (AA) ok = ok & (((ec & my_nx) | (ex & my_nc)) == 0ull);
+                        if constexpr (PA) ok = ok & (en == 0ull || (en & my_nh) != 0ull);
                         // the vote-to-vote path: ballot -> "no fitting lane before me" -> predicated update of S -> next
                         // test.  No branch on it (at the frontier nearly every entry is taken) and no mask arithmetic
                         // beyond one and + compare.
@@ -1019,6 +1077,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                             mask_take(my_nc, ec, loses);
                             mask_take(my_nx, ex, loses);
                         }
+                        if constexpr (PA) mask_take(my_nh, em, loses);
                         note_take(fnd_sa + (unsigned)k, (unsigned)lane, loses);  // off the chain: who took entry k
                         my_takes += loses ? 0u : 1u;
 #pragma unroll
@@ -1027,6 +1086,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         if constexpr (AA) {
                             ec = ec_next;
                             ex = ex_next;
+                        }
+                        if constexpr (PA) {
+                            en = en_next;
+                            em = em_next;
                         }
                     }
                     __syncwarp();
@@ -1050,6 +1113,14 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     if (placed_here >= 0) {  // bookkeeping off the critical path, one lane per placed entry
                         p.placed[(int64_t)(p.tile_lo + tile) * kTile + s_l] = (int32_t)(stage_lo + my_lo + placed_here);
                         atomicAnd(&alive_w[s_l >> 5], ~(1u << (s_l & 31)));
+                        if constexpr (PA) {  // the first placement of a watched signature (rare; never with watch == 0)
+                            unsigned long long w = pm_s[q_l] & p.watch;
+                            if (w) {
+                                const int64_t jj = (int64_t)(p.tile_lo + tile) * kTile + s_l;
+                                const unsigned long long pos = (unsigned long long)(BINS ? (int64_t)p.pod_idx[jj] : jj);
+                                for (; w; w &= w - 1) atomicMin(p.first_placed + (__ffsll((long long)w) - 1), pos);
+                            }
+                        }
                     }
                     head += (unsigned)n_ent;
                     done = endmask != 0;
@@ -1086,6 +1157,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                             nc_s[n] = my_nc;
                             nx_s[n] = my_nx;
                         }
+                        if constexpr (PA) nh_s[n] = my_nh;
                     }
                     if (lane == 0) {
                         if (BINS) opened[warp] = touched_or_open;
@@ -1179,6 +1251,8 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 p.node_carries[stage_lo + n] = nc_s[n];
                 p.node_matches[stage_lo + n] = nx_s[n];
             }
+        if constexpr (PA)
+            for (int n = tid; n < n_valid; n += NT) p.node_has[stage_lo + n] = nh_s[n];
     }
     if (BINS && lane == 0 && my_evals) atomicAdd(p.evals, my_evals);  // every warp credits its own placements
     if (tid == 0) {

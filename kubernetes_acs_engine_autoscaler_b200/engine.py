@@ -170,6 +170,15 @@ class Engine(object):
         self._check(self._lib.acsfit_last_bin_retirement(self._ctx, _ptr(out)))
         return int(out[0]), int(out[1])
 
+    def last_affinity_reruns(self):
+        """test hook: the (signature, position) flips the last pod-affinity call fixed, one per pass it ran again."""
+        n = ctypes.c_int64(0)
+        self._check(self._lib.acsfit_last_affinity_reruns(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p), None))
+        out = np.zeros(2 * n.value, dtype=np.int64)
+        self._check(self._lib.acsfit_last_affinity_reruns(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p),
+                                                          _ptr(out)))
+        return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(n.value)]
+
     def debug_profile(self, enabled=True):
         """developer probe: per-stage clock64 totals [stages, 8] of the last pipeline launch
         (wait, load, scan, resolve, publish, refresh, hits, tiles)."""
@@ -495,6 +504,68 @@ class Engine(object):
             ctypes.cast(ctypes.byref(aa), ctypes.c_void_p), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened),
             _ptr(acc_pool), _ptr(bin_of), ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p),
             ctypes.cast(ctypes.byref(evals), ctypes.c_void_p), self._stream()))
+        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
+                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
+                "evals": int(evals.value)}
+
+    # ------------------------------------------------------------------ pod affinity (include/acsfit.h)
+    def first_fit_nodes_pa(self, req, pod_idx, cap_type, node_type, used, pod_requires, pod_self, pod_matches, node_has,
+                           pod_carries=None, pod_matches_aa=None, node_carries=None, node_matches=None, pod_class=None,
+                           node_match=None, classes=1):
+        """first_fit_nodes with required pod affinity: pod_requires / pod_self / pod_matches uint64 [req rows] device
+        (stored as int64), node_has uint64 [N] device, updated in place like `used`.  The anti-affinity masks (all four
+        or none) and pod_class / node_match (both or neither) as in first_fit_nodes_aa."""
+        rows, D = req.shape
+        P = rows if pod_idx is None else pod_idx.shape[0]
+        N = used.shape[0]
+        placed = self.empty((P,), torch.int32)
+        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
+        sel, keep_s = (None, None) if pod_class is None else \
+            self._selectors(classes, pod_class=pod_class, node_match=node_match)
+        aa, keep_a = (None, None) if pod_carries is None else \
+            self._anti_affinity(pod_carries, pod_matches_aa, node_carries, node_matches)
+        keep_p = [pod_requires, pod_self, pod_matches, node_has]
+        pa = _native.PodAffinity(*[None if a is None else _ptr(a).value for a in keep_p])
+        self._check(self._lib.acsfit_first_fit_nodes_pa(
+            self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
+            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
+            None if aa is None else ctypes.cast(ctypes.byref(aa), ctypes.c_void_p),
+            ctypes.cast(ctypes.byref(pa), ctypes.c_void_p), _ptr(placed), _ptr(decisions), self._stream()))
+        return placed, decisions
+
+    def fulfill_pending_pa(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision,
+                           pod_requires, pod_self, pod_matches, present=0, pod_carries=None, pod_matches_aa=None,
+                           pod_class=None, pool_match=None, classes=1):
+        """fulfill_pending with required pod affinity in the bins: pod_requires / pod_self / pod_matches uint64 [Pp]
+        device (stored as int64); `present` the signatures the nodes already hold (0: only pods this call places
+        count).  The anti-affinity masks (both or neither) and pod_class / pool_match as in fulfill_pending_aa."""
+        Pp, D = req.shape
+        unit = _np(unit, np.float64).reshape(-1, D)
+        T = unit.shape[0]
+        pool_actual = _np(pool_actual, np.int32)
+        pool_max = _np(pool_max, np.int32)
+        pool_ignored = _np(pool_ignored, np.uint8)
+        new_size = np.zeros(T, dtype=np.int64)
+        units_needed = np.zeros(T, dtype=np.int64)
+        bins_opened = np.zeros(T, dtype=np.int64)
+        acc_pool = self.empty((Pp,), torch.int32)
+        bin_of = self.empty((Pp,), torch.int32)
+        unacc = ctypes.c_int64(0)
+        evals = ctypes.c_uint64(0)
+        sel, keep_s = (None, None) if pod_class is None else \
+            self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
+        aa, keep_a = (None, None) if pod_carries is None else self._anti_affinity(pod_carries, pod_matches_aa)
+        keep_p = [pod_requires, pod_self, pod_matches]
+        pa = _native.PodAffinity(*[None if a is None else _ptr(a).value for a in keep_p], None)
+        self._check(self._lib.acsfit_fulfill_pending_pa(
+            self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
+            _ptr(pool_ignored), T, int(over_provision),
+            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
+            None if aa is None else ctypes.cast(ctypes.byref(aa), ctypes.c_void_p),
+            ctypes.cast(ctypes.byref(pa), ctypes.c_void_p), int(present) & 0xFFFFFFFFFFFFFFFF, _ptr(new_size),
+            _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(bin_of),
+            ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p), ctypes.cast(ctypes.byref(evals), ctypes.c_void_p),
+            self._stream()))
         return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
                 "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
                 "evals": int(evals.value)}

@@ -23,7 +23,7 @@ class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                  deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
                  selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False,
-                 anti_affinity_node_states=False):
+                 anti_affinity_node_states=False, pod_affinity=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
@@ -32,6 +32,7 @@ class EngineScaler(Scaler):
         self.node_affinity = node_affinity
         self.pod_anti_affinity = pod_anti_affinity
         self.anti_affinity_node_states = anti_affinity_node_states
+        self.pod_affinity = pod_affinity
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)

@@ -143,22 +143,21 @@ def selector_matches(selector, labels):
     return True
 
 
-def anti_affinity_terms(affinity, namespace, owner):
-    """the required pod anti-affinity terms of spec.affinity that this project honours, as (namespaces, selector)
-    pairs: frozenset of namespaces (empty `namespaces` = the carrying pod's own), canonical label_selector.  Only terms
-    with topologyKey kubernetes.io/hostname count; a term with an absent or null labelSelector selects no pod and a
-    term with a namespaceSelector is not honoured, so both are left out.  ValueError naming the owner when a field
-    is malformed."""
+def _required_pod_terms(affinity, field, namespace, owner):
+    """the required terms of spec.affinity.<field> (podAffinity or podAntiAffinity) with topologyKey
+    kubernetes.io/hostname and no namespaceSelector, as (namespaces, selector) pairs: frozenset of namespaces (empty
+    `namespaces` = the carrying pod's own), canonical label_selector or None for an absent or null labelSelector.
+    ValueError naming the owner when a field is malformed."""
     if affinity is None:
-        return ()
+        return []
     _mapping(affinity, 'spec.affinity', owner)
-    anti = affinity.get('podAntiAffinity')
-    if anti is None:
-        return ()
-    _mapping(anti, 'spec.affinity.podAntiAffinity', owner)
-    what = 'spec.affinity.podAntiAffinity.requiredDuringSchedulingIgnoredDuringExecution'
+    block = affinity.get(field)
+    if block is None:
+        return []
+    _mapping(block, 'spec.affinity.' + field, owner)
+    what = 'spec.affinity.%s.requiredDuringSchedulingIgnoredDuringExecution' % field
     terms = []
-    for t in _entries(anti.get('requiredDuringSchedulingIgnoredDuringExecution'), what, owner):
+    for t in _entries(block.get('requiredDuringSchedulingIgnoredDuringExecution'), what, owner):
         topology = t.get('topologyKey')
         if not isinstance(topology, str):
             raise ValueError("malformed %s entry of %s: topologyKey %r" % (what, owner, topology))
@@ -166,10 +165,34 @@ def anti_affinity_terms(affinity, namespace, owner):
         namespaces = [] if namespaces is None else _str_list(namespaces, what + '.namespaces', owner)
         selector = t.get('labelSelector')
         selector = None if selector is None else label_selector(selector, owner, what + '.labelSelector')
-        if topology != HOSTNAME_TOPOLOGY_KEY or selector is None or t.get('namespaceSelector') is not None:
+        if topology != HOSTNAME_TOPOLOGY_KEY or t.get('namespaceSelector') is not None:
             continue
         terms.append((frozenset(namespaces) if namespaces else frozenset((namespace,)), selector))
-    return tuple(dict.fromkeys(terms))
+    return terms
+
+
+def anti_affinity_terms(affinity, namespace, owner):
+    """the required pod anti-affinity terms of spec.affinity that this project honours, as (namespaces, selector)
+    pairs: frozenset of namespaces (empty `namespaces` = the carrying pod's own), canonical label_selector.  Only terms
+    with topologyKey kubernetes.io/hostname count; a term with an absent or null labelSelector selects no pod and a
+    term with a namespaceSelector is not honoured, so both are left out.  ValueError naming the owner when a field
+    is malformed."""
+    terms = _required_pod_terms(affinity, 'podAntiAffinity', namespace, owner)
+    return tuple(dict.fromkeys(t for t in terms if t[1] is not None))
+
+
+def affinity_terms(affinity, namespace, owner):
+    """the required pod affinity terms of spec.affinity that this project honours, as anti_affinity_terms gives them,
+    except that a term with an absent or null labelSelector is kept with selector None: it selects no pod, so the pod
+    can land nowhere, as in Kubernetes (dropping it would make the pod look placeable).  Terms with another topology
+    key or a namespaceSelector are left out; that never makes a pod harder to place than Kubernetes would."""
+    return tuple(dict.fromkeys(_required_pod_terms(affinity, 'podAffinity', namespace, owner)))
+
+
+def affinity_term_selects(term, namespace, labels):
+    """the pod affinity term (namespaces, selector or None) selects a pod with this namespace and these labels"""
+    namespaces, selector = term
+    return selector is not None and namespace in namespaces and selector_matches(selector, labels)
 
 
 # required node affinity: the operators of a NodeSelectorRequirement, and the one field a matchFields entry may name
@@ -429,6 +452,11 @@ class KubePod(object):
     def anti_affinity_terms(self):
         """the honoured required pod anti-affinity terms (kube.anti_affinity_terms); read on use, like tolerations."""
         return anti_affinity_terms(self.original.obj['spec'].get('affinity'), self.namespace, 'pod %s' % self)
+
+    @property
+    def affinity_terms(self):
+        """the honoured required pod affinity terms (kube.affinity_terms); read on use, like tolerations."""
+        return affinity_terms(self.original.obj['spec'].get('affinity'), self.namespace, 'pod %s' % self)
 
     @property
     def node_affinity(self):

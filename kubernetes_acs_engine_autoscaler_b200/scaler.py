@@ -75,6 +75,8 @@ class Scaler(object):
         # with pod anti-affinity: POD_PENDING only when some pod to schedule could land on the node given the pods
         # already there (Cluster(anti_affinity_node_states=...))
         self.anti_affinity_node_states = False
+        # required pod affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_affinity=...))
+        self.pod_affinity = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -111,8 +113,10 @@ class Scaler(object):
                                     **self.pending_flags([node], [node_pods], pods_to_schedule, node_pods))
         return STATE_NAMES[int(code.cpu().numpy()[0])]
 
-    def fulfill_pending(self, pods):
-        """number of new VMs per pool needed for the pending pods (scaler.py:117-184)."""
+    def fulfill_pending(self, pods, affinity_present=()):
+        """number of new VMs per pool needed for the pending pods (scaler.py:117-184).  `affinity_present`: with pod
+        affinity on, the signatures the nodes already hold (Cluster.affinity_present); without it only the pods this
+        call places count."""
         logger.info("====Scaling for %s pods ====", len(pods))
         # the reference keys its bookkeeping by pod (hash = uid): duplicates collapse onto their first
         # occurrence, but num_unaccounted starts at len(pods) (scaler.py:119-120)
@@ -123,8 +127,10 @@ class Scaler(object):
             classes = snapshot.selector_classes(unique, [], ordered_pools, taints=self.node_taints,
                                                 affinity=self.node_affinity)
         anti_affinity = snapshot.anti_affinity(unique) if self.pod_anti_affinity else None
+        pod_affinity = snapshot.pod_affinity(unique) if self.pod_affinity else None
         res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision,
-                               classes=classes, anti_affinity=anti_affinity)
+                               classes=classes, anti_affinity=anti_affinity, pod_affinity=pod_affinity,
+                               affinity_present=affinity_present)
 
         new_pool_sizes, current_pool_sizes = {}, {}
         unaccounted = len(pods)
@@ -146,6 +152,12 @@ class Scaler(object):
             logger.debug("remaining pending: %s", unaccounted)
         assert unaccounted == res["num_unaccounted"]
 
+        if unaccounted and pod_affinity is not None and logger.isEnabledFor(logging.WARNING):
+            # a pod that no bin of any pool took although it passed the feasibility check: its affinity kept it out
+            for p, t, b, r in zip(unique, acc.tolist(), res["bin_of"].tolist(), pod_affinity.pod_requires.tolist()):
+                if t < 0 and b < 0 and r:
+                    logger.warning("Pending pod %s cannot fit: no node or new node would hold a pod its required pod "
+                                   "affinity selects. Scheduling skipped." % p.name)
         if unaccounted:
             logger.warning('Failed to scale sufficiently.')
             if self.REFERENCE_RAISE_ON_INSUFFICIENT:

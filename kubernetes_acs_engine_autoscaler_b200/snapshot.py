@@ -538,6 +538,87 @@ def _anti_affinity_masks(pods, running, run_idx):
 
 
 # ------------------------------------------------------------------------------------------------
+# required pod affinity: signature masks (include/acsfit.h, acsfit_pod_affinity)
+# ------------------------------------------------------------------------------------------------
+MAX_PA_SIGNATURES = 64
+
+
+class PodAffinity(object):
+    """pod_requires uint64[P] (the bit of the pod's signature, 0 without one), pod_matches uint64[P] (the signatures the
+    pod matches), pod_self = pod_requires & pod_matches, node_has uint64[N] (the OR of pod_matches over the pods already
+    on each node), present (the OR of node_has) and the signatures: bit s = signatures[s], a frozenset of terms."""
+
+    def __init__(self, pod_requires, pod_matches, node_has, signatures):
+        self.pod_requires = pod_requires
+        self.pod_matches = pod_matches
+        self.pod_self = pod_requires & pod_matches
+        self.node_has = node_has
+        self.signatures = signatures
+
+    @property
+    def present(self):
+        """the OR of node_has: the signatures some node holds"""
+        return int(np.bitwise_or.reduce(self.node_has)) if len(self.node_has) else 0
+
+    def present_signatures(self):
+        """the signatures some node holds, as a set (the numbering of another call differs)"""
+        present = self.present
+        return {sig for k, sig in enumerate(self.signatures) if (present >> k) & 1}
+
+    @property
+    def trivial(self):
+        """no pod of this call has a signature: the calls without pod affinity give the same result"""
+        return not self.signatures
+
+
+def pod_affinity(pods, nodes=(), running_pods=()):
+    """signature masks of the pods to place (`pods`) and of the nodes (the pods of `running_pods` on them count, matched
+    by node name as the occupancy count and anti_affinity match them).  A pod's signature is the set of its terms
+    (KubePod.affinity_terms); a pod matches a signature when every term of it selects the pod.  Signatures are numbered
+    in first-occurrence order over `pods`; ValueError above 64.  Each term is evaluated once per distinct (namespace,
+    label values it reads) projection of the pods, as anti_affinity does."""
+    pods, nodes, running = list(pods), list(nodes), list(running_pods)
+    row_ptr, run_idx = running_csr(nodes, running) if nodes and running else (None, np.zeros(0, np.int32))
+    P = len(pods)
+    sig_id, signatures, requires = {}, [], np.zeros(P, dtype=np.uint64)
+    for i, p in enumerate(pods):
+        terms = p.affinity_terms
+        if not terms:
+            continue
+        sig = frozenset(terms)
+        k = sig_id.get(sig)
+        if k is None:
+            if len(signatures) == MAX_PA_SIGNATURES:
+                raise ValueError("more than %d distinct pod affinity signatures are not supported" % MAX_PA_SIGNATURES)
+            k = sig_id[sig] = len(signatures)
+            signatures.append(sig)
+        requires[i] = np.uint64(1) << np.uint64(k)
+    node_has = np.zeros(len(nodes), dtype=np.uint64)
+    if not signatures:
+        return PodAffinity(requires, np.zeros(P, np.uint64), node_has, signatures)
+    on_nodes = np.unique(run_idx)
+    everyone = pods + [running[j] for j in on_nodes.tolist()]
+    terms = list(dict.fromkeys(t for sig in signatures for t in sig))
+    keys = sorted({key for _, sel in terms if sel is not None for key, *_ in sel[0] + sel[1]})
+    group, proj, code_of = _pod_projection(everyone, keys)
+    column = {key: 1 + k for k, key in enumerate(keys)}
+    hit = {t: (_term_selects(t, proj, code_of, column) if t[1] is not None else np.zeros(len(proj), bool))
+           for t in terms}
+    group_matches = np.zeros(len(proj), dtype=np.uint64)
+    for k, sig in enumerate(signatures):
+        both = np.ones(len(proj), bool)
+        for t in sig:
+            both &= hit[t]
+        group_matches[both] |= np.uint64(1) << np.uint64(k)
+    matches = group_matches[group]
+    if len(run_idx):
+        at = P + np.searchsorted(on_nodes, run_idx)
+        node_of = np.repeat(np.arange(len(nodes), dtype=np.int64), np.diff(row_ptr))
+        np.bitwise_or.at(node_has, node_of, matches[at])
+    return PodAffinity(requires, matches[:P].copy(), node_has, signatures)
+
+
+# ------------------------------------------------------------------------------------------------
 # K0: feasibility (capacity.is_possible over the pools)
 # ------------------------------------------------------------------------------------------------
 def feasible_pods(pods, agent_pools, classes=None):
@@ -609,11 +690,12 @@ def count_running_pods(nodes, running_pods):
 # ------------------------------------------------------------------------------------------------
 # first fit over nodes (Cluster.get_pending_pods)
 # ------------------------------------------------------------------------------------------------
-def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None):
+def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None, pod_affinity=None):
     """returns placed[len(pods)] (node index or -1) and mutates node.used_capacity like count_pod.  With `classes`
     (selector_classes(pods, nodes, [])) a pod only takes a node that matches its nodeSelector.  With `anti_affinity`
     (anti_affinity(pods, nodes, running_pods)) a pod only takes a node its required anti-affinity does not block; the
-    node masks are updated in place."""
+    node masks are updated in place.  With `pod_affinity` (pod_affinity(pods, nodes, running_pods)) a pod only takes a
+    node its required pod affinity admits; node_has is updated in place."""
     pods, nodes = list(pods), list(nodes)
     placed = np.full(len(pods), -1, dtype=np.int32)
     if not pods or not nodes:
@@ -628,7 +710,30 @@ def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None):
     eng = get_engine()
     d_used = eng.dev(used, torch.float64)
     sel = classes is not None and not classes.trivial
-    if anti_affinity is not None and not anti_affinity.trivial:
+    if pod_affinity is not None and not pod_affinity.trivial:
+        pa = pod_affinity
+        aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
+        d_nh = eng.dev(pa.node_has.view(np.int64), torch.int64)
+        d_nc = d_nx = None
+        aa_args = ()
+        if aa is not None:
+            d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
+            aa_args = (eng.dev(aa.pod_carries.view(np.int64), torch.int64),
+                       eng.dev(aa.pod_matches.view(np.int64), torch.int64), d_nc, d_nx)
+        d_placed, _ = eng.first_fit_nodes_pa(eng.dev(req, torch.float64),
+                                             None if not bad.any() else eng.dev(ok_idx, torch.int32),
+                                             eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
+                                             eng.dev(pa.pod_requires.view(np.int64), torch.int64),
+                                             eng.dev(pa.pod_self.view(np.int64), torch.int64),
+                                             eng.dev(pa.pod_matches.view(np.int64), torch.int64), d_nh, *aa_args,
+                                             **(dict(pod_class=eng.dev(classes.pod_class, torch.uint8),
+                                                     node_match=eng.dev(classes.node_match.view(np.int64), torch.int64),
+                                                     classes=classes.classes) if sel else {}))
+        pa.node_has[:] = d_nh.cpu().numpy().view(np.uint64)
+        if aa is not None:
+            aa.node_carries[:] = d_nc.cpu().numpy().view(np.uint64)
+            aa.node_matches[:] = d_nx.cpu().numpy().view(np.uint64)
+    elif anti_affinity is not None and not anti_affinity.trivial:
         aa = anti_affinity
         d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
         d_placed, _ = eng.first_fit_nodes_aa(eng.dev(req, torch.float64),
@@ -684,10 +789,13 @@ def single_can_fit(node, resources):
 # fulfill_pending (bins)
 # ------------------------------------------------------------------------------------------------
 def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_provision, classes=None,
-            anti_affinity=None):
+            anti_affinity=None, pod_affinity=None, affinity_present=()):
     """Scaler.fulfill_pending's packing + size arithmetic; pools already in visiting order.  With `classes`
     (selector_classes(unique_pods, [], ordered_pools)) a pool only takes the pods whose nodeSelector it matches.  With
-    `anti_affinity` (anti_affinity(unique_pods)) a pod only takes a bin its required anti-affinity does not block."""
+    `anti_affinity` (anti_affinity(unique_pods)) a pod only takes a bin its required anti-affinity does not block.  With
+    `pod_affinity` (pod_affinity(unique_pods)) a pod only takes a bin its required pod affinity admits;
+    `affinity_present` holds the signatures the nodes already hold (PodAffinity.present_signatures of the node pass);
+    without it only the pods this call places count."""
     from . import capacity
     units = [capacity.RESOURCE_SPEC[pool.instance_type] for pool in ordered_pools]
     dims = Dims([p.resources for p in unique_pods] + units)
@@ -700,7 +808,19 @@ def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_pro
              np.asarray([min(pool.max_size, 2 ** 31 - 1) for pool in ordered_pools], dtype=np.int32),
              np.asarray([1 if pool.name in ignored_pool_names else 0 for pool in ordered_pools], dtype=np.uint8))
     sel = classes is not None and not classes.trivial
-    if anti_affinity is not None and not anti_affinity.trivial:
+    if pod_affinity is not None and not pod_affinity.trivial:
+        pa, aa = pod_affinity, anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
+        present = sum(1 << k for k, sig in enumerate(pa.signatures) if sig in affinity_present)
+        res = eng.fulfill_pending_pa(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
+                                     eng.dev(pa.pod_requires.view(np.int64), torch.int64),
+                                     eng.dev(pa.pod_self.view(np.int64), torch.int64),
+                                     eng.dev(pa.pod_matches.view(np.int64), torch.int64), present,
+                                     *((eng.dev(aa.pod_carries.view(np.int64), torch.int64),
+                                        eng.dev(aa.pod_matches.view(np.int64), torch.int64)) if aa is not None else
+                                       (None, None)),
+                                     *((eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
+                                       if sel else ()))
+    elif anti_affinity is not None and not anti_affinity.trivial:
         res = eng.fulfill_pending_aa(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
                                      eng.dev(anti_affinity.pod_carries.view(np.int64), torch.int64),
                                      eng.dev(anti_affinity.pod_matches.view(np.int64), torch.int64),
