@@ -247,6 +247,30 @@ ACSFIT_API acsfit_status acsfit_pending_admit(acsfit_ctx *ctx, const int64_t *ro
                                               acsfit_stream_t stream);
 
 /*
+ * Pending-pod admission with required pod affinity (opt-in), with or without anti-affinity: acsfit_pending_admit
+ * plus the affinity test.  HAS(n) is the OR of run_has (the pod-affinity signatures each pod matches, acsfit's
+ * pod-affinity numbering) over the pods already on node n.  A signature (class c, carries, matches, need) admits node n
+ * when acsfit_pending_admit's test passes (only the class test when the anti-affinity arrays are NULL) and need == 0 or
+ * (need & HAS(n)) != 0.  need is the pod's signature bit, or 0 for a pod without pod-affinity terms and for the first
+ * pod of a self-affine group (the host folds that exception in: no pod in the cluster matches the signature yet and
+ * the pod matches it itself).
+ *   run_carries, run_matches, sig_carries, sig_matches: all four NULL (the affinity test alone; the anti-affinity
+ *               masks are never read) or given as in acsfit_pending_admit (the run pair may be NULL when there are no
+ *               rows, the signature pair when U == 0)
+ *   run_has     [dev] one mask per row (may be NULL when row_ptr[N] == row_ptr[0])
+ *   sig_need    [host] U masks
+ * The other arguments are those of acsfit_pending_admit.  ACSFIT_E_INVALID: its refusals (with the anti-affinity
+ * test: a NULL run_carries or run_matches when there are rows, a NULL sig_carries or sig_matches when U > 0), a NULL
+ * run_has when there are rows, a NULL sig_need when U > 0, or a misaligned run_has; the flags are then left untouched.  acsfit_last_scan_launch reports the launch as kernel 4.
+ */
+ACSFIT_API acsfit_status acsfit_pending_admit_pa(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
+                                                 const uint64_t *run_matches, const uint64_t *run_has, int64_t N,
+                                                 const uint64_t *node_match, const uint8_t *sig_class,
+                                                 const uint64_t *sig_carries, const uint64_t *sig_matches,
+                                                 const uint64_t *sig_need, int U, uint8_t *node_flags_inout,
+                                                 acsfit_stream_t stream);
+
+/*
  * K6b maintain_actions -- the decision part of EngineScaler.maintain (reference
  * engine_scaler.py:133-182): SPARE_AGENT substitution against the per-pool drain budget
  * (budget0 = actual - len(unschedulable) - spare, :136; it only decrements when not dry_run,
@@ -543,7 +567,9 @@ ACSFIT_API acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, i
  *   {kernel (0 none, 1 occupancy, 2 node states), form (0 per thread, 1 index gather, 2 bulk copy), D,
  *    staging bytes per warp (0 per thread), warps per CTA, table entries per staging chunk (0 per thread),
  *    grid (CTAs), S (idle thresholds; 0 for occupancy)}
- * acsfit_pending_admit reports {3, 0, 0, shared-memory bytes per CTA, warps per CTA, signatures per tile, grid, U}. */
+ * acsfit_pending_admit reports {3, 0, 0, shared-memory bytes per CTA, warps per CTA, signatures per tile, grid, U};
+ * acsfit_pending_admit_pa {4, 1 with the anti-affinity test (0 without), 0, shared-memory bytes per CTA, warps per CTA,
+ * signatures per tile, grid, U}. */
 #define ACSFIT_SCAN_FIELDS 8
 ACSFIT_API acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out);
 

@@ -29,6 +29,8 @@ SIGNATURES = {
     "acsfit_node_states": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int,
                                    c_vp, c_int, c_vp, c_vp]),
     "acsfit_pending_admit": (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp]),
+    "acsfit_pending_admit_pa": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
+                                        c_vp, c_vp]),
     "acsfit_maintain_actions": (c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_vp, c_vp]),
     "acsfit_scale_up": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
                                 c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

@@ -56,7 +56,7 @@ class Cluster(object):
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
                  node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None,
-                 pod_affinity=None):
+                 pod_affinity=None, pod_affinity_node_states=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -106,6 +106,14 @@ class Cluster(object):
         if pod_affinity is None:
             pod_affinity = os.environ.get('ACSFIT_POD_AFFINITY', '0') not in ('', '0')
         self.pod_affinity = bool(pod_affinity)
+        # with pod affinity on, also in maintain: a node is pod-pending only when some pod to schedule could land on it
+        # given its required pod affinity, so a pod that needs a pod elsewhere does not freeze every idle node (opt-in;
+        # None: $ACSFIT_POD_AFFINITY_NODE_STATES).  Combines with selector_node_states and anti_affinity_node_states.
+        if pod_affinity_node_states is None:
+            pod_affinity_node_states = os.environ.get('ACSFIT_POD_AFFINITY_NODE_STATES', '0') not in ('', '0')
+        elif pod_affinity_node_states and not self.pod_affinity:
+            raise ValueError("pod_affinity_node_states=True needs pod_affinity on")
+        self.pod_affinity_node_states = bool(pod_affinity_node_states) and self.pod_affinity
         self.affinity_present = set()  # signatures the last node pass left on some node (scale() hands them on)
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
@@ -209,7 +217,8 @@ class Cluster(object):
             idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
             selector_node_states=self.selector_node_states, node_taints=self.node_taints,
             pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity,
-            anti_affinity_node_states=self.anti_affinity_node_states, pod_affinity=self.pod_affinity)
+            anti_affinity_node_states=self.anti_affinity_node_states, pod_affinity=self.pod_affinity,
+            pod_affinity_node_states=self.pod_affinity_node_states)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [

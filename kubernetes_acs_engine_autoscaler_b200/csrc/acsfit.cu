@@ -2410,6 +2410,83 @@ extern "C" acsfit_status acsfit_node_states(acsfit_ctx *ctx, const int64_t *row_
 
 static bool aligned8(const void *p) { return ((uintptr_t)p & 7u) == 0; }
 
+// acsfit_pending_admit and acsfit_pending_admit_pa: one validation, arena and launch.  `pa` is the entry point (its
+// launch record is kernel 4; acsfit_pending_admit's stays kernel 3).  The anti-affinity test runs when any of the four
+// anti-affinity arrays is given (always, for acsfit_pending_admit); the run pair must then be given when there are rows
+// and the signature pair when U > 0.  The affinity test runs with `pa`.
+static acsfit_status pending_admit_impl(acsfit_ctx *ctx, bool pa, const int64_t *row_ptr,
+                                        const uint64_t *run_carries, const uint64_t *run_matches,
+                                        const uint64_t *run_has, int64_t N, const uint64_t *node_match,
+                                        const uint8_t *sig_class, const uint64_t *sig_carries,
+                                        const uint64_t *sig_matches, const uint64_t *sig_need, int U,
+                                        uint8_t *node_flags_inout, cudaStream_t st)
+{
+    const char *what = pa ? "pending_admit_pa" : "pending_admit";
+    const bool aa = !pa || run_carries || run_matches || sig_carries || sig_matches;
+    if (N < 0 || U < 0 || (N > 0 && (!row_ptr || !node_flags_inout)) ||
+        (N > 0 && U > 0 && (!sig_class || (aa && (!sig_carries || !sig_matches)) || (pa && !sig_need))))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
+    if (N == 0) return ACSFIT_OK;
+    if ((N + kAdmitBlock - 1) / kAdmitBlock > INT32_MAX)
+        return fail(ctx, ACSFIT_E_INVALID, "%s: N=%lld nodes is too many", what, (long long)N);
+    if (!aligned8(row_ptr) || !aligned8(run_carries) || !aligned8(run_matches) || !aligned8(run_has) ||
+        !aligned8(node_match))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: row_ptr and the mask arrays must be 8-byte aligned", what);
+    for (int u = 0; u < U; ++u)
+        if (sig_class[u] >= ACSFIT_MAX_CLASSES)
+            return fail(ctx, ACSFIT_E_INVALID, "%s: signature %d has class %d, need < %d", what, u, sig_class[u],
+                        ACSFIT_MAX_CLASSES);
+    int64_t ends[2] = {0, 0};  // row_ptr[0], row_ptr[N]: the rows the kernel reads
+    CUDA_TRY(cudaMemcpyAsync(&ends[0], row_ptr, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&ends[1], row_ptr + N, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (ends[0] < 0 || ends[1] < ends[0])
+        return fail(ctx, ACSFIT_E_INVALID, "%s: row_ptr[0]=%lld, row_ptr[N]=%lld", what, (long long)ends[0],
+                    (long long)ends[1]);
+    if (ends[1] > ends[0] && ((aa && (!run_carries || !run_matches)) || (pa && !run_has)))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: %lld rows but a NULL run mask array", what,
+                    (long long)(ends[1] - ends[0]));
+    const size_t Uq = (size_t)std::max(U, 1);
+    TRY(arena_reserve(ctx, Uq * ((aa ? 2 : 0) * sizeof(uint64_t) + (pa ? sizeof(uint64_t) : 0) + 1) + 1024, st));
+    ctx->arena_off = 0;
+    unsigned long long *d_carries = nullptr, *d_matches = nullptr, *d_need = nullptr;
+    if (aa) {
+        TAKE(carries, unsigned long long, Uq);
+        TAKE(matches, unsigned long long, Uq);
+        d_carries = carries;
+        d_matches = matches;
+    }
+    if (pa) {
+        TAKE(need, unsigned long long, Uq);
+        d_need = need;
+    }
+    TAKE(d_class, uint8_t, Uq);
+    if (U > 0) {
+        if (aa) {
+            CUDA_TRY(cudaMemcpyAsync(d_carries, sig_carries, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
+            CUDA_TRY(cudaMemcpyAsync(d_matches, sig_matches, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
+        }
+        if (pa) CUDA_TRY(cudaMemcpyAsync(d_need, sig_need, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_class, sig_class, U, cudaMemcpyHostToDevice, st));
+    }
+    const int grid = (int)((N + kAdmitBlock - 1) / kAdmitBlock);
+    auto kernel = !pa ? pending_admit_kernel<true, false>
+                      : aa ? pending_admit_kernel<true, true> : pending_admit_kernel<false, true>;
+    kernel<<<grid, kAdmitBlock, 0, st>>>(
+        row_ptr, reinterpret_cast<const unsigned long long *>(run_carries),
+        reinterpret_cast<const unsigned long long *>(run_matches), N,
+        reinterpret_cast<const unsigned long long *>(node_match), d_class, d_carries, d_matches, U, node_flags_inout,
+        reinterpret_cast<const unsigned long long *>(run_has), d_need);
+    if (pa)
+        ctx->scan_rec = {4, aa ? 1 : 0, 0, aa ? kAdmitSmemAaPa : kAdmitSmemPa, kAdmitBlock / 32, kAdmitBlock, grid, U};
+    else
+        ctx->scan_rec = {3, kScanPerThread, 0, kAdmitSmem, kAdmitBlock / 32, kAdmitBlock, grid, U};
+    ++ctx->launches;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));  // the signature table is a host buffer
+    return ACSFIT_OK;
+}
+
 extern "C" acsfit_status acsfit_pending_admit(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
                                               const uint64_t *run_matches, int64_t N, const uint64_t *node_match,
                                               const uint8_t *sig_class, const uint64_t *sig_carries,
@@ -2417,50 +2494,20 @@ extern "C" acsfit_status acsfit_pending_admit(acsfit_ctx *ctx, const int64_t *ro
                                               acsfit_stream_t stream)
 {
     TRY(enter(ctx, 1));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (N < 0 || U < 0 || (N > 0 && (!row_ptr || !node_flags_inout)) ||
-        (N > 0 && U > 0 && (!sig_class || !sig_carries || !sig_matches)))
-        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: bad arguments");
-    if (N == 0) return ACSFIT_OK;
-    if ((N + kAdmitBlock - 1) / kAdmitBlock > INT32_MAX)
-        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: N=%lld nodes is too many", (long long)N);
-    if (!aligned8(row_ptr) || !aligned8(run_carries) || !aligned8(run_matches) || !aligned8(node_match))
-        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: row_ptr and the mask arrays must be 8-byte aligned");
-    for (int u = 0; u < U; ++u)
-        if (sig_class[u] >= ACSFIT_MAX_CLASSES)
-            return fail(ctx, ACSFIT_E_INVALID, "pending_admit: signature %d has class %d, need < %d", u, sig_class[u],
-                        ACSFIT_MAX_CLASSES);
-    int64_t ends[2] = {0, 0};  // row_ptr[0], row_ptr[N]: the rows the kernel reads
-    CUDA_TRY(cudaMemcpyAsync(&ends[0], row_ptr, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(&ends[1], row_ptr + N, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (ends[0] < 0 || ends[1] < ends[0])
-        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: row_ptr[0]=%lld, row_ptr[N]=%lld", (long long)ends[0],
-                    (long long)ends[1]);
-    if (ends[1] > ends[0] && (!run_carries || !run_matches))
-        return fail(ctx, ACSFIT_E_INVALID, "pending_admit: %lld rows but a NULL run mask array",
-                    (long long)(ends[1] - ends[0]));
-    const size_t Uq = (size_t)std::max(U, 1);
-    TRY(arena_reserve(ctx, Uq * (2 * sizeof(uint64_t) + 1) + 1024, st));
-    ctx->arena_off = 0;
-    TAKE(d_carries, unsigned long long, Uq);
-    TAKE(d_matches, unsigned long long, Uq);
-    TAKE(d_class, uint8_t, Uq);
-    if (U > 0) {
-        CUDA_TRY(cudaMemcpyAsync(d_carries, sig_carries, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_matches, sig_matches, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_class, sig_class, U, cudaMemcpyHostToDevice, st));
-    }
-    const int grid = (int)((N + kAdmitBlock - 1) / kAdmitBlock);
-    pending_admit_kernel<<<grid, kAdmitBlock, 0, st>>>(
-        row_ptr, reinterpret_cast<const unsigned long long *>(run_carries),
-        reinterpret_cast<const unsigned long long *>(run_matches), N,
-        reinterpret_cast<const unsigned long long *>(node_match), d_class, d_carries, d_matches, U, node_flags_inout);
-    ctx->scan_rec = {3, kScanPerThread, 0, kAdmitSmem, kAdmitBlock / 32, kAdmitBlock, grid, U};
-    ++ctx->launches;
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(st));  // the signature table is a host buffer
-    return ACSFIT_OK;
+    return pending_admit_impl(ctx, false, row_ptr, run_carries, run_matches, nullptr, N, node_match, sig_class,
+                              sig_carries, sig_matches, nullptr, U, node_flags_inout, (cudaStream_t)stream);
+}
+
+extern "C" acsfit_status acsfit_pending_admit_pa(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
+                                                 const uint64_t *run_matches, const uint64_t *run_has, int64_t N,
+                                                 const uint64_t *node_match, const uint8_t *sig_class,
+                                                 const uint64_t *sig_carries, const uint64_t *sig_matches,
+                                                 const uint64_t *sig_need, int U, uint8_t *node_flags_inout,
+                                                 acsfit_stream_t stream)
+{
+    TRY(enter(ctx, 1));
+    return pending_admit_impl(ctx, true, row_ptr, run_carries, run_matches, run_has, N, node_match, sig_class,
+                              sig_carries, sig_matches, sig_need, U, node_flags_inout, (cudaStream_t)stream);
 }
 
 static acsfit_status maintain_actions_impl(acsfit_ctx *ctx, uint8_t *io_state, const int32_t *node_pool, int64_t N,

@@ -1,5 +1,6 @@
-// acsfit_admit.cuh -- the pending-pod admission test of node states with pod anti-affinity (acsfit_pending_admit,
-// include/acsfit.h): which nodes some pod to schedule could land on, given the pods already there.
+// acsfit_admit.cuh -- the pending-pod admission test of node states with pod anti-affinity and pod affinity
+// (acsfit_pending_admit, acsfit_pending_admit_pa, include/acsfit.h): which nodes some pod to schedule could land on,
+// given the pods already there.
 #pragma once
 #include <cstdint>
 
@@ -7,30 +8,41 @@ namespace acsfit {
 
 constexpr int kAdmitBlock = 256;  // threads per CTA = nodes per CTA = signatures per shared-memory tile
 constexpr int kAdmitSmem = kAdmitBlock * (2 * 8 + 1);  // static shared bytes per CTA: one tile of the table
+constexpr int kAdmitSmemPa = kAdmitBlock * (8 + 1);    // ... of the pod-affinity-only form (class, need)
+constexpr int kAdmitSmemAaPa = kAdmitBlock * (3 * 8 + 1);  // ... of the combined form (class, carries, matches, need)
 constexpr uint8_t kNodeNoPendingMatch = 2u;  // ACSFIT_NODEF_NO_PENDING_MATCH
 
-// One thread per node.  The thread ORs the carries / matches masks of the node's CSR slice (rows row_ptr[n] ..
-// row_ptr[n+1], absolute), then walks the signature table, which the CTA stages through shared memory one tile at a
-// time.  A signature (class, carries, matches) admits the node when the node matches the class and
-// (carries & NX) | (matches & NC) == 0.  A thread stops testing once a signature admits its node, and the CTA stops
-// loading tiles once every node of it is admitted.  Nodes no signature admits gain the flag bit; no other bit changes.
+// One thread per node.  The thread ORs the masks of the node's CSR slice (rows row_ptr[n] .. row_ptr[n+1], absolute):
+// carries / matches into NC / NX with AA, has into HAS with PA.  It then walks the signature table, which the CTA
+// stages through shared memory one tile at a time.  A signature (class, carries, matches, need) admits the node when
+// the node matches the class, with AA (carries & NX) | (matches & NC) == 0, and with PA need == 0 or
+// (need & HAS) != 0.  A thread stops testing once a signature admits its node, and the CTA stops loading tiles once
+// every node of it is admitted.  Nodes no signature admits gain the flag bit; no other bit changes.  A form reads only
+// the arrays of its tests (the PA-only form never touches the anti-affinity masks).  The PA arrays come last so that
+// the AA-only form keeps the parameter layout it had before pod affinity.
+template <bool AA, bool PA>
 __global__ void __launch_bounds__(kAdmitBlock)
 pending_admit_kernel(const int64_t *__restrict__ row_ptr, const unsigned long long *__restrict__ run_carries,
                      const unsigned long long *__restrict__ run_matches, int64_t N,
                      const unsigned long long *__restrict__ node_match, const uint8_t *__restrict__ sig_class,
                      const unsigned long long *__restrict__ sig_carries,
-                     const unsigned long long *__restrict__ sig_matches, int U, uint8_t *__restrict__ node_flags)
+                     const unsigned long long *__restrict__ sig_matches, int U, uint8_t *__restrict__ node_flags,
+                     const unsigned long long *__restrict__ run_has, const unsigned long long *__restrict__ sig_need)
 {
-    __shared__ unsigned long long s_carries[kAdmitBlock], s_matches[kAdmitBlock];
+    __shared__ unsigned long long s_carries[AA ? kAdmitBlock : 1], s_matches[AA ? kAdmitBlock : 1];
+    __shared__ unsigned long long s_need[PA ? kAdmitBlock : 1];
     __shared__ uint8_t s_class[kAdmitBlock];
     const int t = threadIdx.x;
     const int64_t n = (int64_t)blockIdx.x * kAdmitBlock + t;
-    unsigned long long nc = 0, nx = 0, classes = ~0ull;
+    unsigned long long nc = 0, nx = 0, has = 0, classes = ~0ull;
     bool open = n < N;  // no signature has admitted the node yet
     if (open) {
         for (int64_t k = row_ptr[n], e = row_ptr[n + 1]; k < e; ++k) {
-            nc |= run_carries[k];
-            nx |= run_matches[k];
+            if constexpr (AA) {
+                nc |= run_carries[k];
+                nx |= run_matches[k];
+            }
+            if constexpr (PA) has |= run_has[k];
         }
         if (node_match) classes = node_match[n];
     }
@@ -39,12 +51,17 @@ pending_admit_kernel(const int64_t *__restrict__ row_ptr, const unsigned long lo
         const int cnt = min(kAdmitBlock, U - base);
         if (t < cnt) {
             s_class[t] = sig_class[base + t];
-            s_carries[t] = sig_carries[base + t];
-            s_matches[t] = sig_matches[base + t];
+            if constexpr (AA) {
+                s_carries[t] = sig_carries[base + t];
+                s_matches[t] = sig_matches[base + t];
+            }
+            if constexpr (PA) s_need[t] = sig_need[base + t];
         }
         __syncthreads();
         for (int j = 0; open && j < cnt; ++j)
-            if (((classes >> s_class[j]) & 1ull) && ((s_carries[j] & nx) | (s_matches[j] & nc)) == 0) open = false;
+            if (((classes >> s_class[j]) & 1ull) && (!AA || ((s_carries[j] & nx) | (s_matches[j] & nc)) == 0) &&
+                (!PA || s_need[j] == 0 || (s_need[j] & has) != 0))
+                open = false;
     }
     if (open) node_flags[n] |= kNodeNoPendingMatch;
 }

@@ -279,6 +279,25 @@ class Engine(object):
                                                    _ptr(sig_matches), U, _ptr(node_flags), self._stream()))
         return node_flags
 
+    def pending_admit_pa(self, row_ptr, run_carries, run_matches, run_has, node_match, sig_class, sig_carries,
+                         sig_matches, sig_need, node_flags):
+        """pending_admit with the pod-affinity test (include/acsfit.h, acsfit_pending_admit_pa): a signature (class,
+        carries, matches, need) admits a node only when need is 0 or the node's pods match some signature of need too.
+        run_has uint64 [rows] (stored as int64) on the device; sig_need a host array of length U.  run_carries,
+        run_matches, sig_carries and sig_matches are all None (no anti-affinity test) or all given."""
+        N = node_flags.shape[0]
+        sig_class, sig_need = _np(sig_class, np.uint8), _np(sig_need, np.uint64)
+        U = sig_class.shape[0]
+        assert sig_need.shape == (U,)
+        if sig_carries is not None or sig_matches is not None:
+            sig_carries, sig_matches = _np(sig_carries, np.uint64), _np(sig_matches, np.uint64)
+            assert sig_carries.shape == sig_matches.shape == (U,)
+        self._check(self._lib.acsfit_pending_admit_pa(self._ctx, _ptr(row_ptr), _ptr(run_carries), _ptr(run_matches),
+                                                      _ptr(run_has), N, _ptr(node_match), _ptr(sig_class),
+                                                      _ptr(sig_carries), _ptr(sig_matches), _ptr(sig_need), U,
+                                                      _ptr(node_flags), self._stream()))
+        return node_flags
+
     def maintain_actions(self, state, node_pool, budget0, pool_scalable, dry_run):
         """engine_scaler.py:133-182 decisions. `state` uint8[N] device is rewritten; returns action uint8[N]."""
         N = state.shape[0]

@@ -23,7 +23,7 @@ class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                  deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
                  selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False,
-                 anti_affinity_node_states=False, pod_affinity=False):
+                 anti_affinity_node_states=False, pod_affinity=False, pod_affinity_node_states=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
@@ -33,6 +33,7 @@ class EngineScaler(Scaler):
         self.pod_anti_affinity = pod_anti_affinity
         self.anti_affinity_node_states = anti_affinity_node_states
         self.pod_affinity = pod_affinity
+        self.pod_affinity_node_states = pod_affinity_node_states
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)
@@ -120,7 +121,8 @@ class EngineScaler(Scaler):
             lists = [pods_by_node.get(node.name, []) for node in nodes]
             state_dev = snapshot.node_states(nodes, lists, bool(pods_to_schedule), self.idle_threshold,
                                              **self.pending_flags(nodes, lists, pods_to_schedule,
-                                                                  running_or_pending_assigned_pods))
+                                                                  running_or_pending_assigned_pods,
+                                                                  agent_pools=self.agent_pools))
             states, actions = snapshot.maintain_actions(state_dev, node_pool, budget0, [1] * len(budget0),
                                                         self.dry_run)
             info = logger.isEnabledFor(logging.INFO)  # (formatted eagerly, as upstream: skipped when nobody listens)

@@ -77,6 +77,9 @@ class Scaler(object):
         self.anti_affinity_node_states = False
         # required pod affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_affinity=...))
         self.pod_affinity = False
+        # with pod affinity: POD_PENDING only when some pod to schedule could land on the node given its required pod
+        # affinity (Cluster(pod_affinity_node_states=...))
+        self.pod_affinity_node_states = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -91,23 +94,31 @@ class Scaler(object):
             return None
         return ~snapshot.pending_match(pods_to_schedule, nodes, taints=self.node_taints, affinity=self.node_affinity)
 
-    def pending_flags(self, nodes, pods_lists, pods_to_schedule, running_pods):
-        """the keywords `no_match` and `admit` of snapshot.node_states.  With anti_affinity_node_states on, something
-        to schedule and some anti-affinity term that can block a pod to schedule, the GPU decides which nodes some pod
-        to schedule is admitted to (snapshot.pending_admit, node selectors included when selector_node_states is on);
-        otherwise no_pending_match decides."""
+    def pending_flags(self, nodes, pods_lists, pods_to_schedule, running_pods, agent_pools=None):
+        """the keywords `no_match` and `admit` of snapshot.node_states.  With anti_affinity_node_states or
+        pod_affinity_node_states on, something to schedule and some term that can exclude a pod to schedule, the GPU
+        decides which nodes some pod to schedule is admitted to (snapshot.pending_admit: the enabled tests, node
+        selectors included when selector_node_states is on); otherwise no_pending_match decides.  A self-affine group
+        may bootstrap while no pod of `running_pods` on a node of `agent_pools` matches it (None: no pod of
+        `pods_lists`)."""
         admit = None
-        if self.anti_affinity_node_states and pods_to_schedule:
+        if (self.anti_affinity_node_states or self.pod_affinity_node_states) and pods_to_schedule:
+            agent_nodes = None
+            if self.pod_affinity_node_states and agent_pools is not None:
+                agent_nodes = [n for pool in agent_pools for n in pool.nodes]
             admit = snapshot.pending_admit(pods_to_schedule, running_pods, nodes, pods_lists,
                                            selectors=self.selector_node_states, taints=self.node_taints,
-                                           affinity=self.node_affinity)
+                                           affinity=self.node_affinity, anti_affinity=self.anti_affinity_node_states,
+                                           pod_affinity=self.pod_affinity_node_states, agent_nodes=agent_nodes)
         if admit is not None:
             return {"no_match": None, "admit": admit}
         return {"no_match": self.no_pending_match(nodes, pods_to_schedule), "admit": None}
 
     def get_node_state(self, node, node_pods, pods_to_schedule):
         """ClusterNodeState of one node (scaler.py:61-114): a one-node launch of the idle scan.
-        EngineScaler.maintain classifies all nodes in a single launch instead."""
+        EngineScaler.maintain classifies all nodes in a single launch instead.  The anti-affinity and pod-affinity
+        rules see only `node_pods`: with pod_affinity_node_states on, a self-affine group may bootstrap here unless one
+        of `node_pods` matches it, whereas maintain looks for a match on every agent node."""
         node_pods = list(node_pods)
         code = snapshot.node_states([node], [node_pods], bool(pods_to_schedule), self.idle_threshold,
                                     **self.pending_flags([node], [node_pods], pods_to_schedule, node_pods))

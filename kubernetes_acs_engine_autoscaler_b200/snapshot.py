@@ -466,13 +466,19 @@ def anti_affinity_rows(pods, running_pods, pods_lists):
     their numbering and their dropping are then those of anti_affinity(pods, nodes, running_pods).  Raises ValueError
     for a pod of `pods_lists` that is not in `running_pods`."""
     running = list(running_pods)
+    return _anti_affinity_masks(list(pods), running, _row_index(running, pods_lists))
+
+
+def _row_index(running, pods_lists):
+    """int64[R]: the index in `running` of every pod of the concatenated `pods_lists` (matched by identity); ValueError
+    for a pod that is not in `running`"""
     ids = np.fromiter(map(id, running), dtype=np.int64, count=len(running))
     order = np.argsort(ids, kind="stable")
     flat = np.fromiter(map(id, itertools.chain.from_iterable(pods_lists)), dtype=np.int64)
     pos = np.searchsorted(ids[order], flat)
     if len(flat) and ((pos >= len(ids)).any() or (ids[order[np.minimum(pos, len(ids) - 1)]] != flat).any()):
         raise ValueError("a pod of pods_lists is not one of running_pods")
-    return _anti_affinity_masks(list(pods), running, order[pos] if len(flat) else np.zeros(0, np.int64))
+    return order[pos] if len(flat) else np.zeros(0, np.int64)
 
 
 def _anti_affinity_masks(pods, running, run_idx):
@@ -579,6 +585,40 @@ def pod_affinity(pods, nodes=(), running_pods=()):
     label values it reads) projection of the pods, as anti_affinity does."""
     pods, nodes, running = list(pods), list(nodes), list(running_pods)
     row_ptr, run_idx = running_csr(nodes, running) if nodes and running else (None, np.zeros(0, np.int32))
+    requires, matches, run_matches, signatures = _pod_affinity_masks(pods, running, run_idx)
+    node_has = np.zeros(len(nodes), dtype=np.uint64)
+    if len(run_idx) and signatures:
+        node_of = np.repeat(np.arange(len(nodes), dtype=np.int64), np.diff(row_ptr))
+        np.bitwise_or.at(node_has, node_of, run_matches)
+    return PodAffinity(requires, matches, node_has, signatures)
+
+
+def pod_affinity_rows(pods, running_pods, pods_lists, nodes=None):
+    """pod_affinity's masks for maintain's table: (pod_requires uint64[P], pod_self uint64[P], pod_matches uint64[P],
+    row_has uint64[R], present, signatures).  row_has holds the signatures each entry of the concatenated `pods_lists`
+    (node_states' table; objects of `running_pods`) matches, before the OR per node.  `present` (an int) is the OR of
+    the signatures matched by the pods of `running_pods` on `nodes` (matched by node name, as pod_affinity matches
+    them), or by the rows of the table when `nodes` is None: the pods whose presence ends a self-affine group's
+    bootstrap.  The signatures and their numbering are those of pod_affinity(pods, nodes, running_pods).  Raises
+    ValueError for a pod of `pods_lists` that is not in `running_pods`."""
+    pods, running = list(pods), list(running_pods)
+    rows = _row_index(running, pods_lists)
+    if nodes is None:
+        on_nodes = np.zeros(0, np.int64)
+    else:
+        names = {n.name for n in nodes}
+        on_nodes = np.fromiter((j for j, p in enumerate(running) if p.node_name in names), dtype=np.int64)
+    requires, matches, run_matches, signatures = _pod_affinity_masks(pods, running, np.concatenate([rows, on_nodes]))
+    row_has = run_matches[:len(rows)]
+    seen = row_has if nodes is None else run_matches[len(rows):]
+    present = int(np.bitwise_or.reduce(seen)) if len(seen) else 0
+    return requires, requires & matches, matches, row_has, present, signatures
+
+
+def _pod_affinity_masks(pods, running, run_idx):
+    """(pod_requires[P], pod_matches[P], run_matches, signatures): the signature masks of the pods to place and the
+    signatures running[run_idx[k]] matches for every k, for pod_affinity and pod_affinity_rows.  Each term is
+    evaluated once over the pods to place and the running pods run_idx names."""
     P = len(pods)
     sig_id, signatures, requires = {}, [], np.zeros(P, dtype=np.uint64)
     for i, p in enumerate(pods):
@@ -593,9 +633,8 @@ def pod_affinity(pods, nodes=(), running_pods=()):
             k = sig_id[sig] = len(signatures)
             signatures.append(sig)
         requires[i] = np.uint64(1) << np.uint64(k)
-    node_has = np.zeros(len(nodes), dtype=np.uint64)
     if not signatures:
-        return PodAffinity(requires, np.zeros(P, np.uint64), node_has, signatures)
+        return requires, np.zeros(P, np.uint64), np.zeros(len(run_idx), np.uint64), signatures
     on_nodes = np.unique(run_idx)
     everyone = pods + [running[j] for j in on_nodes.tolist()]
     terms = list(dict.fromkeys(t for sig in signatures for t in sig))
@@ -611,11 +650,8 @@ def pod_affinity(pods, nodes=(), running_pods=()):
             both &= hit[t]
         group_matches[both] |= np.uint64(1) << np.uint64(k)
     matches = group_matches[group]
-    if len(run_idx):
-        at = P + np.searchsorted(on_nodes, run_idx)
-        node_of = np.repeat(np.arange(len(nodes), dtype=np.int64), np.diff(row_ptr))
-        np.bitwise_or.at(node_has, node_of, matches[at])
-    return PodAffinity(requires, matches[:P].copy(), node_has, signatures)
+    at = P + np.searchsorted(on_nodes, run_idx)  # a running pod is in `everyone` at P + its rank in on_nodes
+    return requires, matches[:P].copy(), matches[at], signatures
 
 
 # ------------------------------------------------------------------------------------------------
@@ -887,44 +923,71 @@ def node_age_seconds(node, now_by_tz=None):
 
 
 class PendingAdmit(object):
-    """what acsfit_pending_admit reads beside node_states' table: row_carries / row_matches uint64[R] (one per row of the
-    table), node_match uint64[N] class masks or None (every pod matches every node), and the U distinct signatures
-    (class, carries, matches) of the pods to schedule: sig_class uint8[U], sig_carries / sig_matches uint64[U]."""
+    """what acsfit_pending_admit(_pa) reads beside node_states' table: row_carries / row_matches uint64[R] (one per row
+    of the table; None without the anti-affinity test), row_has uint64[R] (None without the pod-affinity test),
+    node_match uint64[N] class masks or None (every pod matches every node), and the U distinct signatures (class,
+    carries, matches, need) of the pods to schedule: sig_class uint8[U], sig_carries / sig_matches / sig_need uint64[U]
+    (None without the test they belong to)."""
 
-    def __init__(self, row_carries, row_matches, node_match, sig_class, sig_carries, sig_matches):
+    def __init__(self, row_carries, row_matches, node_match, sig_class, sig_carries, sig_matches, row_has=None,
+                 sig_need=None):
         self.row_carries = row_carries
         self.row_matches = row_matches
         self.node_match = node_match
         self.sig_class = sig_class
         self.sig_carries = sig_carries
         self.sig_matches = sig_matches
+        self.row_has = row_has
+        self.sig_need = sig_need
 
 
-def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints=False, affinity=False):
+def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints=False, affinity=False,
+                  anti_affinity=True, pod_affinity=False, agent_nodes=None):
     """the PendingAdmit of node_states(admit=...): node n stays pod-pending only when some pod of `pods` (the pods to
-    schedule) is blocked by no pod of pods_lists[n] (the node's pods, objects of `running_pods`) in either direction,
-    and, with `selectors`, matches the node as pending_match(pods, nodes, taints, affinity) decides.  The masks are
-    anti_affinity_rows'; the classes selector_classes(pods, nodes, [], taints, affinity)'s (ValueError above 64).
-    None when no term is kept: nothing can block a pod to schedule, and pending_match alone decides."""
+    schedule) passes every enabled test against pods_lists[n] (the node's pods, objects of `running_pods`):
+    * `anti_affinity`: no pod of the node blocks it and it blocks none of them (anti_affinity_rows' masks);
+    * `pod_affinity`: it has no pod-affinity signature, or some pod of the node matches its signature, or it may
+      bootstrap a self-affine group: it matches its own signature and no pod of `running_pods` on `agent_nodes` does
+      (pod_affinity_rows' masks; `agent_nodes` None: the pods of the table).  The bootstrap is folded into the need:
+      need = 0 when requires & present == 0 and self != 0, need = requires otherwise;
+    * `selectors`: it matches the node as pending_match(pods, nodes, taints, affinity) decides (the classes are
+      selector_classes(pods, nodes, [], taints, affinity)'s; ValueError above 64).
+    None when no enabled test can exclude a pod to schedule (no anti-affinity term is kept and no need is nonzero):
+    pending_match alone decides.  Without a nonzero need the table is the anti-affinity one (acsfit_pending_admit)."""
     pods = list(pods)
-    pod_carries, pod_matches, row_carries, row_matches, terms = anti_affinity_rows(pods, running_pods, pods_lists)
-    if not terms:
+    row_carries = row_matches = row_has = None
+    columns = []
+    if anti_affinity:
+        pod_carries, pod_matches, rc, rm, terms = anti_affinity_rows(pods, running_pods, pods_lists)
+        if terms:
+            row_carries, row_matches = rc, rm
+            columns += [pod_carries, pod_matches]
+    if pod_affinity:
+        requires, own, _, rh, present, _ = pod_affinity_rows(pods, running_pods, pods_lists, nodes=agent_nodes)
+        need = np.where(((requires & np.uint64(present)) == 0) & (own != 0), np.uint64(0), requires)
+        if need.any():
+            row_has = rh
+            columns.append(need)
+    if not columns:
         return None
     pod_class, node_match = np.zeros(len(pods), dtype=np.uint8), None
     if selectors:
         classes = selector_classes(pods, nodes, [], taints=taints, affinity=affinity)
         if not classes.trivial:
             pod_class, node_match = classes.pod_class, classes.node_match
-    sig = np.unique(np.stack([pod_class.astype(np.uint64), pod_carries, pod_matches], axis=1), axis=0)
-    return PendingAdmit(row_carries, row_matches, node_match, sig[:, 0].astype(np.uint8),
-                        np.ascontiguousarray(sig[:, 1]), np.ascontiguousarray(sig[:, 2]))
+    sig = np.unique(np.stack([pod_class.astype(np.uint64)] + columns, axis=1), axis=0)
+    col = lambda k: np.ascontiguousarray(sig[:, k])  # noqa: E731
+    aa = row_carries is not None
+    return PendingAdmit(row_carries, row_matches, node_match, sig[:, 0].astype(np.uint8), col(1) if aa else None,
+                        col(2) if aa else None, row_has, col(len(columns)) if row_has is not None else None)
 
 
 def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None, admit=None):
     """state code per node (include/acsfit.h ACSFIT_ST_*); pods_lists[n] = the node's pods in order.  `no_match`
     (bool[N], optional): nodes no pod to schedule matches (~pending_match); they are classified as if there were no
     pod to schedule (ACSFIT_NODEF_NO_PENDING_MATCH).  `admit` (pending_admit(..., pods_lists=pods_lists), optional):
-    the same flag for the nodes that no pod to schedule is admitted to, set on the GPU (acsfit_pending_admit)."""
+    the same flag for the nodes that no pod to schedule is admitted to, set on the GPU (acsfit_pending_admit, or
+    acsfit_pending_admit_pa when the table has row_has)."""
     nodes = list(nodes)
     if not nodes:
         return np.zeros(0, dtype=np.uint8)
@@ -946,12 +1009,18 @@ def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None, a
     eng = get_engine()
     d_row_ptr, d_node_flags = eng.dev(row_ptr, torch.int64), eng.dev(node_flags, torch.uint8)
     if admit is not None:
-        if len(admit.row_carries) != len(flat):
-            raise ValueError("pending_admit masks of %d pods for a table of %d" % (len(admit.row_carries), len(flat)))
-        eng.pending_admit(d_row_ptr, eng.dev(admit.row_carries.view(np.int64), torch.int64),
-                          eng.dev(admit.row_matches.view(np.int64), torch.int64),
-                          None if admit.node_match is None else eng.dev(admit.node_match.view(np.int64), torch.int64),
-                          admit.sig_class, admit.sig_carries, admit.sig_matches, d_node_flags)
+        rows = admit.row_carries if admit.row_carries is not None else admit.row_has
+        if len(rows) != len(flat):
+            raise ValueError("pending_admit masks of %d pods for a table of %d" % (len(rows), len(flat)))
+        dev_masks = lambda a: None if a is None else eng.dev(a.view(np.int64), torch.int64)  # noqa: E731
+        if admit.row_has is None:
+            eng.pending_admit(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
+                              dev_masks(admit.node_match), admit.sig_class, admit.sig_carries, admit.sig_matches,
+                              d_node_flags)
+        else:
+            eng.pending_admit_pa(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
+                                 dev_masks(admit.row_has), dev_masks(admit.node_match), admit.sig_class,
+                                 admit.sig_carries, admit.sig_matches, admit.sig_need, d_node_flags)
     st = eng.node_states(d_row_ptr,
                          None,  # contiguous table: the rows ARE in node order (bulk-copy streaming kernel)
                          eng.dev(req_run, torch.float64), eng.dev(flags, torch.uint8),

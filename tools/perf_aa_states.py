@@ -1,12 +1,14 @@
 #!/usr/bin/env python3
-"""developer probe: cost of node states with pod anti-affinity (Cluster(anti_affinity_node_states=True)).
+"""developer probe: cost of node states with pod anti-affinity and pod affinity (Cluster(anti_affinity_node_states=True),
+Cluster(pod_affinity_node_states=True)).
 
-  kernel   acsfit_pending_admit at --nodes nodes holding --rows running-pod rows, for each U of --sigs, on two tables:
-           `typical` (signature u carries and is selected by term u % 64; half the running pods belong to one of 64
-           such deployments, so most nodes are admitted by one of the first signatures) and `none` (no signature admits
-           any node with pods: every thread walks the whole table).  Per call: median CUDA-event time of the entry
-           point (table upload, row_ptr read-back, kernel) over --reps calls after --warmup; per kernel: the device
-           time torch.profiler records for pending_admit_kernel in a separate run.
+  kernel   for each form of --forms (`aa`: acsfit_pending_admit; `pa`: acsfit_pending_admit_pa without the anti-affinity
+           masks; `aa+pa`: acsfit_pending_admit_pa with them) at --nodes nodes holding --rows running-pod rows, for each
+           U of --sigs, on two tables: `typical` (signature u carries, is selected by and needs term / signature u % 64;
+           half the running pods belong to one of 64 such deployments, so most nodes are admitted by one of the first
+           signatures) and `none` (no signature admits any node with pods: every thread walks the whole table).  Per
+           call: median CUDA-event time of the entry point (table upload, row_ptr read-back, kernel) over --reps calls
+           after --warmup; per kernel: the device time torch.profiler records for pending_admit_kernel in a separate run.
   host     snapshot.pending_admit for U pods to schedule against the same number of running pods and nodes (CPU
            only): term numbering, masks per running pod, the signature table.  Building the pod objects is not timed.
 Prints the GPU and its power limit, read in the same run.
@@ -35,7 +37,7 @@ def gpu_info():
 
 
 def table(N, R, U, kind, seed=5):
-    """row_ptr, run_carries, run_matches, sig_class, sig_carries, sig_matches"""
+    """row_ptr, run_carries, run_matches, run_has, sig_class, sig_carries, sig_matches, sig_need"""
     rng = np.random.default_rng(seed)
     cuts = np.sort(rng.integers(0, R + 1, size=N - 1))
     row_ptr = np.concatenate([[0], cuts, [R]]).astype(np.int64)
@@ -44,14 +46,18 @@ def table(N, R, U, kind, seed=5):
         dep = rng.integers(0, 64, size=R).astype(np.uint64)
         rc = np.where(rng.random(R) < 0.5, np.uint64(1) << dep, np.uint64(0))
         rm = rc.copy()
+        rh = rc.copy()
         car = np.uint64(1) << (u % 64).astype(np.uint64)
         mat = car | (np.uint64(1) << (u // 64 % 64).astype(np.uint64))
+        need = car.copy()
     else:
         rc = np.zeros(R, np.uint64)
         rm = np.ones(R, np.uint64)
+        rh = np.zeros(R, np.uint64)
         car = np.ones(U, np.uint64)
         mat = (u.astype(np.uint64) + np.uint64(1)) << np.uint64(1)  # distinct signatures, all blocked by bit 0
-    return row_ptr, rc, rm, np.zeros(U, np.uint8), car, mat
+        need = np.ones(U, np.uint64)  # and none held
+    return row_ptr, rc, rm, rh, np.zeros(U, np.uint8), car, mat, need
 
 
 def kernel(args):
@@ -59,14 +65,20 @@ def kernel(args):
     from kubernetes_acs_engine_autoscaler_b200.engine import Engine
     eng = Engine(0)
     i64 = torch.int64
-    for kind in ("typical", "none"):
+    for form, kind in ((f, k) for f in args.forms for k in ("typical", "none")):
         for U in args.sigs:
-            row_ptr, rc, rm, cls, car, mat = table(args.nodes, args.rows, U, kind)
+            row_ptr, rc, rm, rh, cls, car, mat, need = table(args.nodes, args.rows, U, kind)
             d_rp, d_rc, d_rm = eng.dev(row_ptr, i64), eng.dev(rc.view(np.int64), i64), eng.dev(rm.view(np.int64), i64)
+            d_rh = eng.dev(rh.view(np.int64), i64)
             flags = eng.dev(np.zeros(args.nodes, np.uint8), torch.uint8)
 
             def call():
-                eng.pending_admit(d_rp, d_rc, d_rm, None, cls, car, mat, flags)
+                if form == "aa":
+                    eng.pending_admit(d_rp, d_rc, d_rm, None, cls, car, mat, flags)
+                elif form == "pa":
+                    eng.pending_admit_pa(d_rp, None, None, d_rh, None, cls, None, None, need, flags)
+                else:
+                    eng.pending_admit_pa(d_rp, d_rc, d_rm, d_rh, None, cls, car, mat, need, flags)
             for _ in range(args.warmup):
                 call()
             times = []
@@ -83,8 +95,8 @@ def kernel(args):
                     call()
                 torch.cuda.synchronize()
             dev_us = [e.self_device_time_total / e.count for e in prof.key_averages() if "pending_admit_kernel" in e.key]
-            print("kernel %-7s N=%d rows=%d U=%-5d call %.3f ms (median of %d)  kernel %s  flagged %d" % (
-                kind, args.nodes, args.rows, U, statistics.median(times), args.reps,
+            print("kernel %-5s %-7s N=%d rows=%d U=%-5d call %.3f ms (median of %d)  kernel %s  flagged %d" % (
+                form, kind, args.nodes, args.rows, U, statistics.median(times), args.reps,
                 "%.3f ms" % (dev_us[0] / 1000.0) if dev_us else "n/a", flagged), flush=True)
 
 
@@ -124,6 +136,7 @@ def main():
     ap.add_argument("--nodes", type=int, default=1_000_000)
     ap.add_argument("--rows", type=int, default=10_000_000)
     ap.add_argument("--sigs", type=int, nargs="+", default=[1, 64, 4096])
+    ap.add_argument("--forms", nargs="+", choices=("aa", "pa", "aa+pa"), default=["aa", "pa", "aa+pa"])
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
