@@ -498,6 +498,68 @@ ACSFIT_API acsfit_status acsfit_fulfill_pending_pa(acsfit_ctx *ctx, const double
  * signature, out_flips[2k + 1] = position (fulfill: pending position; 2 * *out_reruns entries; may be NULL) */
 ACSFIT_API acsfit_status acsfit_last_affinity_reruns(const acsfit_ctx *ctx, int64_t *out_reruns, int64_t *out_flips);
 
+/*
+ * Hostname topology spread (opt-in): spec.topologySpreadConstraints with topologyKey kubernetes.io/hostname and
+ * whenUnsatisfiable DoNotSchedule (at most one per pod).  The host numbers the distinct keys (namespace, selector with
+ * the matchLabelKeys values, domain set) of the pods to place, at most ACSFIT_MAX_TS_KEYS, bit k = key k.
+ *   cnt(k, n)     the pods on node n that key k's selector selects; the pass adds 1 for every key of pod_matches
+ *                 when it places a pod.  A new bin starts at 0
+ *   min(k)        the smallest cnt(k, n) over k's domains: the nodes with bit k in node_domain, and the domains
+ *                 outside the node list (non-agent nodes) whose smallest count the host folds into floor[k]
+ *                 (INT32_MAX: none; 0 when k has fewer domains than its minDomains)
+ *   rule          a pod with pod_key = k (0xFF: none) may take node n only when cnt(k, n) <= pod_skew + min(k),
+ *                 pod_skew = maxSkew - (1 if k's selector selects the pod itself else 0) >= 0.  In the bins min(k) is
+ *                 taken as 0 (a scale-up's new nodes join empty), so a new node takes at most maxSkew self-selecting
+ *                 pods of a key, which may ask for more nodes than the scheduler needs, never fewer.  ANDs with
+ *                 resources, `sel`, `aa` and `pa`; counters otherwise unchanged
+ *   exactness     min(k) rises as the node pass places pods.  The pass runs with a level per key and position, which
+ *                 rises at the fixed rise positions; it watches each key's next rise (every domain of the list at
+ *                 level + 1, unless floor[k] is below that), and the earliest rise or pod-affinity flip it observes is
+ *                 fixed and the pass run again from its saved state: exact after 1 + rises + flips passes, and after
+ *                 one pass when no key can rise (acsfit_last_spread_rises).  After 4096 fixed rises in one call
+ *                 no further rise is watched: the rest of the pass keeps the last fixed levels, which are at most the
+ *                 true minimums (the pass then refuses pods the scheduler would place, and is no longer exact)
+ *   pod_key, pod_skew, pod_matches   [dev] one per row of req
+ *   node_count    [dev] keys x N (key-major), read and written (node pass only; fulfill ignores it)
+ *   node_domain   [dev] N (node pass only)
+ *   floor         [host] keys (node pass only)
+ * acsfit_first_fit_nodes_ts / acsfit_fulfill_pending_ts take the arguments of the *_pa forms with `sel`, `aa` and `pa`
+ * all allowed to be NULL, plus `ts`.  They run the pod-affinity form of the pipeline kernel with the spread test
+ * added, and refuse with ACSFIT_E_INVALID: a NULL `ts` or array that is read, keys outside [0, 64], a pod_key >= keys
+ * other than 0xFF, a pod_matches bit at or above keys, a negative pod_skew, node count or floor, the checks of `sel`, `aa` and `pa`, and cluster mode.
+ */
+#define ACSFIT_MAX_TS_KEYS 64
+typedef struct acsfit_topology_spread {
+    const uint8_t *pod_key;        /* [dev] one per row of req: the pod's key, 0xFF none */
+    const int32_t *pod_skew;       /* [dev] one per row of req: maxSkew - self */
+    const uint64_t *pod_matches;   /* [dev] one per row of req: the keys whose selector selects the pod */
+    int32_t *node_count;           /* [dev] keys x N, in/out (node pass only) */
+    const uint64_t *node_domain;   /* [dev] N: the keys each node is a domain of (node pass only) */
+    const int32_t *floor;          /* [host] keys (node pass only) */
+    int32_t keys;
+} acsfit_topology_spread;
+
+ACSFIT_API acsfit_status acsfit_first_fit_nodes_ts(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                   const int32_t *node_type, double *used_inout, int64_t N,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, const acsfit_topology_spread *ts,
+                                                   int32_t *out_placed, uint64_t *out_decisions, acsfit_stream_t stream);
+ACSFIT_API acsfit_status acsfit_fulfill_pending_ts(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                   int64_t num_listed, int D, const double *unit,
+                                                   const int32_t *pool_actual, const int32_t *pool_max,
+                                                   const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, uint64_t present,
+                                                   const acsfit_topology_spread *ts, int64_t *out_new_size,
+                                                   int64_t *out_units_needed, int64_t *out_bins_opened,
+                                                   int32_t *out_acc_pool, int32_t *out_bin_of,
+                                                   int64_t *out_unaccounted, uint64_t *out_evals,
+                                                   acsfit_stream_t stream);
+/* test hook: the rises the last *_ts call fixed, in order: out_pairs[2k] = key, out_pairs[2k + 1] = position (the
+ * node pass's list entry after which the key's minimum rose; 2 * *out_rises entries; may be NULL) */
+ACSFIT_API acsfit_status acsfit_last_spread_rises(const acsfit_ctx *ctx, int64_t *out_rises, int64_t *out_pairs);
+
 /* acsfit_occupancy_host = acsfit_occupancy with host buffers (reference cluster.py:165-168): R rows of req_run,
  * used_inout N x D is read, updated and written back. */
 ACSFIT_API acsfit_status acsfit_occupancy_host(acsfit_ctx *ctx, const int64_t *row_ptr, const int32_t *run_idx,

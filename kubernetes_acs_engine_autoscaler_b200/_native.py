@@ -75,6 +75,14 @@ SIGNATURES = {
                                           c_vp, c_vp, c_vp, ctypes.c_uint64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                           c_vp]),
     "acsfit_last_affinity_reruns": (c_int, [c_vp, c_vp, c_vp]),
+    # topology spread: the arguments of the _pa form (sel, aa and pa may be NULL) plus a
+    # `const acsfit_topology_spread *` (fulfill: after `present`)
+    "acsfit_first_fit_nodes_ts": (c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "acsfit_fulfill_pending_ts": (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64,
+                                          c_vp, c_vp, c_vp, ctypes.c_uint64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                          c_vp, c_vp]),
+    "acsfit_last_spread_rises": (c_int, [c_vp, c_vp, c_vp]),
 }
 
 
@@ -92,6 +100,12 @@ class AntiAffinity(ctypes.Structure):
 class PodAffinity(ctypes.Structure):
     """struct acsfit_pod_affinity (include/acsfit.h)"""
     _fields_ = [("pod_requires", c_vp), ("pod_self", c_vp), ("pod_matches", c_vp), ("node_has", c_vp)]
+
+
+class TopologySpread(ctypes.Structure):
+    """struct acsfit_topology_spread (include/acsfit.h)"""
+    _fields_ = [("pod_key", c_vp), ("pod_skew", c_vp), ("pod_matches", c_vp), ("node_count", c_vp),
+                ("node_domain", c_vp), ("floor", c_vp), ("keys", ctypes.c_int32)]
 
 
 # one record of acsfit_last_launches (ACSFIT_LAUNCH_FIELDS ints), field names in order

@@ -56,7 +56,7 @@ class Cluster(object):
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
                  node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None,
-                 pod_affinity=None, pod_affinity_node_states=None):
+                 pod_affinity=None, pod_affinity_node_states=None, topology_spread=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -115,6 +115,13 @@ class Cluster(object):
             raise ValueError("pod_affinity_node_states=True needs pod_affinity on")
         self.pod_affinity_node_states = bool(pod_affinity_node_states) and self.pod_affinity
         self.affinity_present = set()  # signatures the last node pass left on some node (scale() hands them on)
+        # honour topologySpreadConstraints with topologyKey kubernetes.io/hostname and whenUnsatisfiable DoNotSchedule in
+        # first fit and bin packing, so that replicas spread over nodes are not simulated onto one roomy node (opt-in;
+        # None: $ACSFIT_TOPOLOGY_SPREAD).  Independent of the other switches.
+        if topology_spread is None:
+            topology_spread = os.environ.get('ACSFIT_TOPOLOGY_SPREAD', '0') not in ('', '0')
+        self.topology_spread = bool(topology_spread)
+        self.other_nodes = []  # the listed nodes that are not agents (the master): domains of the spread constraints
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
         self.service_principal_tenant_id = service_principal_tenant_id
@@ -208,7 +215,10 @@ class Cluster(object):
         if not pykube_nodes:
             logger.warning('Failed to list nodes. Please check kube configuration. Terminating scale loop.')
             return False
-        all_nodes = [n for n in map(self.create_kube_node, pykube_nodes) if utils.is_agent(n)]
+        listed = list(map(self.create_kube_node, pykube_nodes))
+        all_nodes = [n for n in listed if utils.is_agent(n)]
+        # with topology spread on, the scheduler counts the master among a constraint's domains
+        self.other_nodes = [n for n in listed if not utils.is_agent(n)] if self.topology_spread else []
 
         scaler = EngineScaler(
             resource_group=self.resource_group, nodes=all_nodes, deployments=self.deployments,
@@ -218,7 +228,7 @@ class Cluster(object):
             selector_node_states=self.selector_node_states, node_taints=self.node_taints,
             pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity,
             anti_affinity_node_states=self.anti_affinity_node_states, pod_affinity=self.pod_affinity,
-            pod_affinity_node_states=self.pod_affinity_node_states)
+            pod_affinity_node_states=self.pod_affinity_node_states, topology_spread=self.topology_spread)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [
@@ -246,7 +256,8 @@ class Cluster(object):
         """sequential first fit of the pods over the nodes (cluster.py:184-204); placed pods are
         counted into node.used_capacity, the rest are returned in order.
 
-        With pod anti-affinity on, `running_pods` are the pods already on the nodes (the tick's running or assigned
+        With topology spread on, `running_pods` also give each node's count and the non-agent nodes of the tick's listing
+        (self.other_nodes) count as domains.  With pod anti-affinity on, `running_pods` are the pods already on the nodes (the tick's running or assigned
         pending pods, which scale() passes): their terms block pods, and pods' terms block them.  Without it, only the
         pods this call places count.  With pod affinity on they are also what a pod's affinity can find on a node, and
         the signatures the nodes hold afterwards are kept in self.affinity_present for the bin packing."""
@@ -260,8 +271,11 @@ class Cluster(object):
         pod_affinity = None
         if self.pod_affinity:
             pod_affinity = snapshot.pod_affinity(pods, nodes, running_pods or [])
+        topology_spread = None
+        if self.topology_spread:
+            topology_spread = snapshot.topology_spread(pods, nodes, running_pods or [], self.other_nodes)
         placed = snapshot.first_fit_nodes(pods, nodes, classes=classes, anti_affinity=anti_affinity,
-                                          pod_affinity=pod_affinity)
+                                          pod_affinity=pod_affinity, topology_spread=topology_spread)
         self.affinity_present = pod_affinity.present_signatures() if pod_affinity is not None else set()
         detail = len(pods) <= LOG_DETAIL_LIMIT
         pending_pods = []

@@ -55,6 +55,7 @@ struct acsfit_ctx {
     unsigned long long *retire_dev = nullptr;           // [2] dead warps / retired stages of the last call's bin passes
     bool retire_counted = false;                        // retire_dev was zeroed by a bin pass of the last call (acsfit_last_bin_retirement)
     std::vector<int64_t> pa_flips;                      // (signature, position) fixed by the last *_pa call, one per rerun
+    std::vector<int64_t> ts_rises;                      // (key, position) fixed by the last *_ts call, one per rerun
     // launch records of the current API call (acsfit_last_launches); rec_* are set by the caller of a pipeline launch
     std::vector<std::array<int, ACSFIT_LAUNCH_FIELDS>> launch_log;
     int rec_chained = 0, rec_pool = -1;
@@ -412,6 +413,69 @@ __global__ void pa_check_kernel(const unsigned long long *requires_, const unsig
         bad |= (r & (r - 1)) != 0 || (self[i] & ~r) != 0;
     }
     if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 4);
+}
+
+// topology spread: the rises of the keys' minimums fixed so far, as the positions of each key's rises in ascending
+// order (key k: pos[off[k]] .. pos[off[k + 1] - 1]): a pod at position p of key k sees the level base[k] + #{fixed
+// rises of k at positions < p}
+struct TsLevels {
+    int base[64];
+    int off[65];
+    const long long *pos;  // [off[64]] (device)
+};
+// topology spread: the limit of the pod at each position i < n (row idx ? idx[i] : i), maxSkew - self + its key's
+// level there, saturated at INT_MAX (a count never exceeds the pods placed, so a saturated limit never blocks)
+__global__ void ts_lim_kernel(const uint8_t *key, const int32_t *skew, const int32_t *idx, int64_t n, const TsLevels lv,
+                              int32_t *lim)
+{
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t row = idx ? idx[i] : i;
+        const unsigned k = key[row];
+        long long l = skew[row];
+        if (k < 64u) {
+            int lo = lv.off[k], hi = lv.off[k + 1];  // binary search: the rises of k before position i
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (lv.pos[mid] < i) lo = mid + 1;
+                else hi = mid;
+            }
+            l += lv.base[k] + (lo - lv.off[k]);
+        }
+        lim[i] = (int32_t)min(l, (long long)INT_MAX);
+    }
+}
+// topology spread, over the N nodes: target == nullptr: out_min[k] = min of the counts of k's domains, out_ndom[k] =
+// their number; otherwise out_reached[k] = k's domains whose count is >= target[k]
+__global__ void ts_domains_kernel(const int32_t *count, const unsigned long long *domain, int64_t N, int keys,
+                                  const int *target, int *out_min, int *out_ndom, int *out_reached)
+{
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < N * keys; i += (int64_t)gridDim.x * blockDim.x) {
+        const int k = (int)(i / N);
+        const int64_t n = i - (int64_t)k * N;
+        if (!((domain[n] >> k) & 1ull)) continue;
+        const int c = count[i];
+        if (target) {
+            if (c >= target[k]) atomicAdd(out_reached + k, 1);
+        } else {
+            atomicMin(out_min + k, c);
+            atomicAdd(out_ndom + k, 1);
+        }
+    }
+}
+// topology spread: flag[0] |= 8 for a pod_key >= keys (other than 0xFF), a negative pod_skew or a pod_matches bit at or
+// above keys, |= 16 for a negative node count
+__global__ void ts_check_kernel(const uint8_t *key, const int32_t *skew, const unsigned long long *matches, int64_t rows,
+                                int keys, const int32_t *count, int64_t counts, int *flag)
+{
+    const unsigned long long outside = keys >= 64 ? 0ull : ~((1ull << keys) - 1ull);
+    int bad = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows || i < counts;
+         i += (int64_t)gridDim.x * blockDim.x) {
+        if (i < rows) bad |= ((key[i] != 0xFF && key[i] >= keys) || skew[i] < 0 || (matches[i] & outside) != 0) ? 8 : 0;
+        if (i < counts) bad |= count[i] < 0 ? 16 : 0;
+    }
+    for (int o = 16; o > 0; o >>= 1) bad |= __shfl_down_sync(0xFFFFFFFFu, bad, o);
+    if ((threadIdx.x & 31) == 0 && bad) atomicOr(flag, bad);
 }
 
 // domain check: requests must be >= 0 and not NaN; flag[0] |= 1 otherwise
@@ -1004,6 +1068,14 @@ extern "C" acsfit_status acsfit_last_affinity_reruns(const acsfit_ctx *ctx, int6
     return ACSFIT_OK;
 }
 
+extern "C" acsfit_status acsfit_last_spread_rises(const acsfit_ctx *ctx, int64_t *out_rises, int64_t *out_pairs)
+{
+    if (!ctx || !out_rises) return ACSFIT_E_INVALID;
+    *out_rises = (int64_t)ctx->ts_rises.size() / 2;
+    if (out_pairs) std::copy(ctx->ts_rises.begin(), ctx->ts_rises.end(), out_pairs);
+    return ACSFIT_OK;
+}
+
 extern "C" acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out)
 {
     static_assert(sizeof(ScanLaunch) == sizeof(int) * ACSFIT_SCAN_FIELDS, "one int per record field");
@@ -1207,22 +1279,22 @@ static acsfit_status launch_stream(acsfit_ctx *ctx, const PipelineParams &pp, in
 constexpr int kOneCtaSmemKb = 116;  // more than half of the 227 KB an SM offers: a second CTA cannot be resident
 // SEL: the node-selector form of a node pass, AA: the anti-affinity form of a node or bin pass (barrier form only:
 // both ignore the "stream" knob)
-template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false, bool AA = false, bool PA = false>
+template <int D, bool BINS, bool PRUNE, int RW, bool SEL = false, bool AA = false, bool PA = false, bool TS = false>
 static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
     if constexpr (RW > 0 && D <= 8 && !PRUNE && !SEL && !AA) {
         if (stream_form_ok(ctx, D, RW, pp.Tn)) return launch_stream<D, BINS, RW>(ctx, pp, stages, st, resident);
     }
     constexpr int NT = stage_threads(D, BINS);
-    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL, AA, PA>::bytes(pp.Tn);
+    size_t smem = PipelineSmem<D, BINS, NT, PRUNE, RW, SEL, AA, PA, TS>::bytes(pp.Tn, TS ? pp.ts_keys : 0);
     // D >= 8: ONE stage CTA per SM.  Whether two fit is an accident of the register allocation (the bins kernel has
     // been compiled to 128 and to 237 registers by neighbouring source revisions); at c3 a second CTA on the
     // frontier's SM costs the placement chain more than the extra resident stages give back.
     if (D >= 8) smem = std::max(smem, (size_t)kOneCtaSmemKb * 1024);
     if (ctx->smem_floor_kb > 0) smem = std::max(smem, (size_t)ctx->smem_floor_kb * 1024);  // occupancy knob
-    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL, AA, PA>;
+    auto kern = firstfit_pipeline_kernel<D, BINS, NT, PRUNE, RW, SEL, AA, PA, TS>;
     if (resident) {  // only asked: how many stages does the GPU hold at once?  (cached: the query costs ~10 us)
-        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0) | (AA ? 8 : 0) | (PA ? 16 : 0), RW, pp.Tn);
+        const auto key = std::make_tuple(D, (int)BINS, (int)PRUNE | (SEL ? 4 : 0) | (AA ? 8 : 0) | (PA ? 16 : 0) | (TS ? 32 + (pp.ts_keys << 6) : 0), RW, pp.Tn);
         auto it = ctx->resident_cache.find(key);
         if (it == ctx->resident_cache.end()) {
             int per_sm = 0;
@@ -1237,7 +1309,7 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
     PipelineParams q = pp;
     // more stages than the GPU holds at once: several waves, each streaming the whole pod list (see the kernel's publish)
     int held = 0;
-    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA, PA>(ctx, pp, stages, st, &held)));
+    TRY((launch_pipeline_w<D, BINS, PRUNE, RW, SEL, AA, PA, TS>(ctx, pp, stages, st, &held)));
     q.publish_every = (held > 0 && stages > held) ? kPublishEvery : 1;
     q.retire = BINS && ctx->retire;
     if (BINS && RW > 0) {  // the first counted bin pass of a call zeroes the counters (in stream order before the later ones)
@@ -1260,40 +1332,42 @@ static acsfit_status launch_pipeline_w(acsfit_ctx *ctx, const PipelineParams &pp
 }
 
 // the instantiation is chosen by the rank layout of the call: 0 (float64 scan), 1, 2 or 4 packed words per row
-template <int D, bool BINS, bool PRUNE, bool SEL = false, bool AA = false, bool PA = false>
+template <int D, bool BINS, bool PRUNE, bool SEL = false, bool AA = false, bool PA = false, bool TS = false>
 static acsfit_status launch_pipeline_v(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st, int *resident)
 {
     switch (pp.rk.nw) {
-    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL, AA, PA>(ctx, pp, stages, st, resident);
-    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL, AA, PA>(ctx, pp, stages, st, resident);
-    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL, AA, PA>(ctx, pp, stages, st, resident);
-    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL, AA, PA>(ctx, pp, stages, st, resident);
+    case 0: return launch_pipeline_w<D, BINS, PRUNE, 0, SEL, AA, PA, TS>(ctx, pp, stages, st, resident);
+    case 1: return launch_pipeline_w<D, BINS, PRUNE, 1, SEL, AA, PA, TS>(ctx, pp, stages, st, resident);
+    case 2: return launch_pipeline_w<D, BINS, PRUNE, 2, SEL, AA, PA, TS>(ctx, pp, stages, st, resident);
+    case 4: return launch_pipeline_w<D, BINS, PRUNE, 4, SEL, AA, PA, TS>(ctx, pp, stages, st, resident);
     default: return fail(ctx, ACSFIT_E_INVALID, "rank layout with %d words", pp.rk.nw);
     }
 }
 
 // node pass with node selectors (pp.node_match != nullptr), AA: and anti-affinity masks, PA: and pod-affinity masks:
 // the same pruning rule as below, barrier form only
-template <int D, bool AA = false, bool PA = false>
+template <int D, bool AA = false, bool PA = false, bool TS = false>
 static acsfit_status launch_pipeline_sel(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
     int prune = ctx->prune;
     if (prune < 0) {
         int resident = 0;
-        TRY((launch_pipeline_v<D, false, false, true, AA, PA>(ctx, pp, stages, st, &resident)));
+        TRY((launch_pipeline_v<D, false, false, true, AA, PA, TS>(ctx, pp, stages, st, &resident)));
         prune = stages > resident;
     }
-    if (prune) return launch_pipeline_v<D, false, true, true, AA, PA>(ctx, pp, stages, st, nullptr);
-    return launch_pipeline_v<D, false, false, true, AA, PA>(ctx, pp, stages, st, nullptr);
+    if (prune) return launch_pipeline_v<D, false, true, true, AA, PA, TS>(ctx, pp, stages, st, nullptr);
+    return launch_pipeline_v<D, false, false, true, AA, PA, TS>(ctx, pp, stages, st, nullptr);
 }
 
 template <int D, bool BINS>
 static acsfit_status launch_pipeline_t(acsfit_ctx *ctx, const PipelineParams &pp, int stages, cudaStream_t st)
 {
     if constexpr (BINS) {
+        if (pp.ts_key) return launch_pipeline_v<D, true, false, false, true, true, true>(ctx, pp, stages, st, nullptr);
         if (pp.pod_need) return launch_pipeline_v<D, true, false, false, true, true>(ctx, pp, stages, st, nullptr);
         if (pp.pod_carries) return launch_pipeline_v<D, true, false, false, true>(ctx, pp, stages, st, nullptr);
     } else {
+        if (pp.ts_key) return launch_pipeline_sel<D, true, true, true>(ctx, pp, stages, st);  // the entry point set node_match
         if (pp.pod_need) return launch_pipeline_sel<D, true, true>(ctx, pp, stages, st);  // the entry point set node_match
         if (pp.pod_carries) return launch_pipeline_sel<D, true>(ctx, pp, stages, st);  // the entry point set node_match
         if (pp.node_match) return launch_pipeline_sel<D>(ctx, pp, stages, st);
@@ -1729,6 +1803,7 @@ static void reset_stats(acsfit_ctx *ctx)
     ctx->last_sel_hits = 0;
     ctx->retire_counted = false;
     ctx->pa_flips.clear();
+    ctx->ts_rises.clear();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1797,13 +1872,178 @@ static acsfit_status or_rows(acsfit_ctx *ctx, const uint64_t *v, const int32_t *
     return ACSFIT_OK;
 }
 
+// topology spread: one pass's levels, targets and device scratch (include/acsfit.h, acsfit_topology_spread)
+constexpr int kMaxSpreadRises = 4096;  // rises one node pass may fix (each costs a rerun of the pass)
+struct TsPass {
+    const acsfit_topology_spread *ts = nullptr;
+    int32_t *lim = nullptr;                     // [positions]
+    int *target = nullptr, *reached = nullptr;  // [64] each
+    unsigned long long *rise_pos = nullptr;     // [64]
+    int *dmin = nullptr, *dndom = nullptr;      // [64] each
+    long long *rises_dev = nullptr;             // [kMaxSpreadRises]: the fixed rises' positions, per key ascending
+    int base[64], ndom[64], tgt[64], nfixed[64];
+    std::vector<long long> rises;               // fixed (key, position) pairs
+    bool watching = false;                      // some key's next rise is watched in the current pass
+};
+
+static size_t ts_scratch(int64_t positions)
+{
+    return sizeof(int32_t) * (size_t)positions + sizeof(int) * 64 * 4 + sizeof(unsigned long long) * 64 +
+           sizeof(long long) * kMaxSpreadRises + 2048;
+}
+
+static acsfit_status ts_alloc(acsfit_ctx *ctx, const acsfit_topology_spread *ts, int64_t positions, TsPass &tp)
+{
+    tp.ts = ts;
+    tp.lim = arena_take<int32_t>(ctx, (size_t)std::max<int64_t>(1, positions));
+    tp.target = arena_take<int>(ctx, 64);
+    tp.reached = arena_take<int>(ctx, 64);
+    tp.dmin = arena_take<int>(ctx, 64);
+    tp.dndom = arena_take<int>(ctx, 64);
+    tp.rise_pos = arena_take<unsigned long long>(ctx, 64);
+    tp.rises_dev = arena_take<long long>(ctx, kMaxSpreadRises);
+    if (!tp.lim || !tp.target || !tp.reached || !tp.dmin || !tp.dndom || !tp.rise_pos || !tp.rises_dev)
+        return fail(ctx, ACSFIT_E_NOMEM, "scratch arena too small for topology spread");
+    for (int k = 0; k < 64; ++k) {
+        tp.base[k] = 0;
+        tp.ndom[k] = 0;
+        tp.tgt[k] = INT_MAX;
+        tp.nfixed[k] = 0;
+    }
+    return ACSFIT_OK;
+}
+
+// node pass: each key's minimum at the start, min(floor, the smallest count of its domains in the list), and its
+// number of domains in the list
+static acsfit_status ts_begin_nodes(acsfit_ctx *ctx, TsPass &tp, int64_t N, cudaStream_t st)
+{
+    const acsfit_topology_spread *ts = tp.ts;
+    int init[128];
+    for (int k = 0; k < 64; ++k) {
+        init[k] = INT_MAX;
+        init[64 + k] = 0;
+    }
+    CUDA_TRY(cudaMemcpyAsync(tp.dmin, init, sizeof(int) * 64, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(tp.dndom, init + 64, sizeof(int) * 64, cudaMemcpyHostToDevice, st));
+    if (N > 0 && ts->keys > 0) {
+        ts_domains_kernel<<<grid_for(ctx, N * ts->keys, 256), 256, 0, st>>>(
+            ts->node_count, reinterpret_cast<const unsigned long long *>(ts->node_domain), N, ts->keys, nullptr,
+            tp.dmin, tp.dndom, nullptr);
+        ++ctx->launches;
+    }
+    int dmin[64];
+    CUDA_TRY(cudaMemcpyAsync(dmin, tp.dmin, sizeof dmin, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(tp.ndom, tp.dndom, sizeof tp.ndom, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    for (int k = 0; k < ts->keys; ++k) tp.base[k] = std::min(ts->floor[k], dmin[k]);
+    return ACSFIT_OK;
+}
+
+// before a pass: the limits of positions [0, n) under the fixed rises and (node pass) the watch of each key's next
+// rise: its target is its current top level + 1, unless the key has no domain in the list or its floor (the fixed
+// domains outside it) is below the target -- then its minimum can never reach it.  Once kMaxSpreadRises rises are
+// fixed nothing is watched any more: the pass keeps the levels it has, which are at most the true minimums, so beyond
+// the last fixed rise it refuses some pods the scheduler would place and accepts none it would refuse on that count
+static acsfit_status ts_prepare(acsfit_ctx *ctx, TsPass &tp, const int32_t *idx, int64_t n, int64_t N, bool nodes,
+                                cudaStream_t st)
+{
+    const acsfit_topology_spread *ts = tp.ts;
+    tp.watching = false;
+    for (int k = 0; k < 64; ++k) {
+        tp.tgt[k] = INT_MAX;
+        if (!nodes || k >= ts->keys) continue;
+        const long long t = (long long)tp.base[k] + tp.nfixed[k] + 1;
+        if (tp.ndom[k] > 0 && t < INT_MAX && (long long)ts->floor[k] >= t &&
+            (int)tp.rises.size() / 2 < kMaxSpreadRises) {
+            tp.tgt[k] = (int)t;
+            tp.watching = true;
+        }
+    }
+    if (nodes) {
+        CUDA_TRY(cudaMemcpyAsync(tp.target, tp.tgt, sizeof tp.tgt, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemsetAsync(tp.reached, 0, sizeof(int) * 64, st));
+        CUDA_TRY(cudaMemsetAsync(tp.rise_pos, 0, sizeof(unsigned long long) * 64, st));
+        if (tp.watching && N > 0) {  // domains already at the target count as reached
+            ts_domains_kernel<<<grid_for(ctx, N * ts->keys, 256), 256, 0, st>>>(
+                ts->node_count, reinterpret_cast<const unsigned long long *>(ts->node_domain), N, ts->keys, tp.target,
+                nullptr, nullptr, tp.reached);
+            ++ctx->launches;
+        }
+    }
+    TsLevels lv;
+    const int n_rises = (int)tp.rises.size() / 2;
+    std::vector<long long> pos(n_rises);
+    for (int k = 0; k < 64; ++k) {
+        lv.base[k] = tp.base[k];
+        lv.off[k] = 0;
+    }
+    lv.off[64] = 0;
+    for (int r = 0; r < n_rises; ++r) ++lv.off[tp.rises[2 * r] + 1];
+    for (int k = 0; k < 64; ++k) lv.off[k + 1] += lv.off[k];
+    int fill[64];
+    std::copy(lv.off, lv.off + 64, fill);
+    for (int r = 0; r < n_rises; ++r) pos[fill[tp.rises[2 * r]]++] = tp.rises[2 * r + 1];
+    for (int k = 0; k < 64; ++k) std::sort(pos.begin() + lv.off[k], pos.begin() + lv.off[k + 1]);  // (fixed in order)
+    lv.pos = tp.rises_dev;
+    if (n_rises > 0)
+        CUDA_TRY(cudaMemcpyAsync(tp.rises_dev, pos.data(), sizeof(long long) * n_rises, cudaMemcpyHostToDevice, st));
+    if (n > 0) {
+        ts_lim_kernel<<<grid_for(ctx, n, 256), 256, 0, st>>>(ts->pod_key, ts->pod_skew, idx, n, lv, tp.lim);
+        ++ctx->launches;
+    }
+    CUDA_TRY(cudaGetLastError());
+    if (n_rises > 0) CUDA_TRY(cudaStreamSynchronize(st));  // the host copy of the rises must outlive the transfer
+    return ACSFIT_OK;
+}
+
+// after a node pass with topology spread: the earliest event among the placed watched pod-affinity signatures and
+// the keys whose every domain reached its target (the lower event on a tie, a flip before a rise, then the lowest
+// signature / key) is fixed and `again` set; `again` stays false when there is none
+static acsfit_status ts_next_event(acsfit_ctx *ctx, const unsigned long long *first_placed, uint64_t watch,
+                                   uint64_t &fixed, PaFlips &fl, TsPass &tp, bool &again, cudaStream_t st)
+{
+    again = false;
+    const uint64_t open = watch & ~fixed;
+    unsigned long long fp[64], rp[64];
+    int reached[64];
+    if (open) CUDA_TRY(cudaMemcpyAsync(fp, first_placed, sizeof fp, cudaMemcpyDeviceToHost, st));
+    if (tp.watching) {
+        CUDA_TRY(cudaMemcpyAsync(rp, tp.rise_pos, sizeof rp, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(reached, tp.reached, sizeof reached, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(st));
+    int best_s = -1, best_k = -1;
+    for (int s = 0; open && s < 64; ++s)
+        if (((open >> s) & 1u) && fp[s] != ~0ull && (best_s < 0 || fp[s] < fp[best_s])) best_s = s;
+    for (int k = 0; tp.watching && k < 64; ++k)
+        if (tp.tgt[k] != INT_MAX && reached[k] >= tp.ndom[k] && (best_k < 0 || rp[k] < rp[best_k])) best_k = k;
+    if (best_s >= 0 && (best_k < 0 || fp[best_s] <= rp[best_k])) {
+        fl.f[best_s] = (long long)fp[best_s];
+        fixed |= 1ull << best_s;
+        ctx->pa_flips.push_back(best_s);
+        ctx->pa_flips.push_back((int64_t)fp[best_s]);
+        again = true;
+    } else if (best_k >= 0) {  // (ts_prepare watches nothing once kMaxSpreadRises are fixed)
+        tp.rises.push_back(best_k);
+        tp.rises.push_back((long long)rp[best_k]);
+        ++tp.nfixed[best_k];
+        ctx->ts_rises.push_back(best_k);
+        ctx->ts_rises.push_back((int64_t)rp[best_k]);
+        again = true;
+    }
+    return ACSFIT_OK;
+}
+
 // aa (needs pod_class / node_match): anti-affinity masks (the SEL + AA form; single GPU only)
 // pa (needs aa): pod-affinity masks (the SEL + AA + PA form), run again from the saved node state per fixed flip
+// ts (needs pa): topology spread (the SEL + AA + PA + TS form), run again per fixed flip or rise
 static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const int32_t *pod_idx, int64_t P, int D,
                                     const double *cap_type, const int32_t *node_type, double *used, int64_t N,
                                     int32_t *out_placed, unsigned long long *out_decisions, cudaStream_t st,
                                     const uint8_t *pod_class = nullptr, const unsigned long long *node_match = nullptr,
-                                    const acsfit_anti_affinity *aa = nullptr, const acsfit_pod_affinity *pa = nullptr)
+                                    const acsfit_anti_affinity *aa = nullptr, const acsfit_pod_affinity *pa = nullptr,
+                                    const acsfit_topology_spread *ts = nullptr)
 {
     if (ctx->world > 1)
         return cluster_first_fit(ctx, req, pod_idx, P, D, cap_type, node_type, used, N, out_placed, out_decisions, st);
@@ -1862,8 +2102,27 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
     }
     // pod affinity: the signatures no node holds at the start that some pod of the list matches itself are watched;
     // the pass runs again, from the saved node state, for every one that gets placed (include/acsfit.h)
+    // topology spread: the keys' minimums at the start, the watched next rises and the limits of the first pass
+    TsPass tp;
+    int32_t *counts0 = nullptr;
+    if (ts) {
+        TRY(ts_alloc(ctx, ts, P, tp));
+        TRY(ts_begin_nodes(ctx, tp, N, st));
+        TRY(ts_prepare(ctx, tp, pod_idx, P, N, true, st));
+        pp.ts_key = ts->pod_key;
+        pp.ts_lim = tp.lim;
+        pp.ts_matches = reinterpret_cast<const unsigned long long *>(ts->pod_matches);
+        pp.ts_count = ts->node_count;
+        pp.ts_domain = reinterpret_cast<const unsigned long long *>(ts->node_domain);
+        pp.ts_target = tp.target;
+        pp.ts_reached = tp.reached;
+        pp.ts_rise_pos = tp.rise_pos;
+        pp.ts_stride = N;
+        pp.ts_keys = ts->keys;
+    }
     PaFlips fl;
     uint64_t watch = 0, fixed = 0;
+    bool rerun = false;  // a later pass may be needed: the node state is saved
     double *used0 = nullptr;
     unsigned long long *masks0 = nullptr, *need = nullptr;
     if (pa) {
@@ -1879,7 +2138,13 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
         TRY(or_rows(ctx, pa->pod_self, pod_idx, P, nullptr, red, &selfs, st));
         for (int s = 0; s < 64; ++s) fl.f[s] = ((present >> s) & 1u) ? -1 : INT64_MAX;
         watch = selfs & ~present;
-        if (watch) {
+        rerun = watch || (ts && tp.watching);
+        if (ts && rerun && ts->keys > 0) {  // the counts change in a pass: a rerun starts from the saved ones
+            counts0 = arena_take<int32_t>(ctx, (size_t)N * ts->keys);
+            if (!counts0) return fail(ctx, ACSFIT_E_NOMEM, "scratch arena too small for topology spread");
+            CUDA_TRY(cudaMemcpyAsync(counts0, ts->node_count, sizeof(int32_t) * N * ts->keys, cudaMemcpyDeviceToDevice, st));
+        }
+        if (rerun) {
             used0 = arena_take<double>(ctx, (size_t)N * D);
             masks0 = arena_take<unsigned long long>(ctx, (size_t)N * 3);
             if (!used0 || !masks0) return fail(ctx, ACSFIT_E_NOMEM, "scratch arena too small for pod affinity");
@@ -1894,10 +2159,11 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
 
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
     TRY(launch_pipeline<false>(ctx, D, pp, plan.stages, st));
-    for (bool again = pa && watch;;) {
+    for (bool again = pa && rerun;;) {
         if (again) {
             TRY(check_pipeline_status(ctx, status, st));
-            TRY(pa_next_flip(ctx, pp.first_placed, watch, fixed, fl, again, st));
+            if (ts) TRY(ts_next_event(ctx, pp.first_placed, watch, fixed, fl, tp, again, st));
+            else TRY(pa_next_flip(ctx, pp.first_placed, watch, fixed, fl, again, st));
         }
         if (!again) break;
         // run the pass again from its start: node state, sync words, alive bits and placements
@@ -1911,6 +2177,11 @@ static acsfit_status first_fit_impl(acsfit_ctx *ctx, const double *req, const in
         ctx->launches += 2;
         pp.watch = watch & ~fixed;
         TRY(pa_prepare(ctx, pa, pod_idx, P, fl, pp.watch, need, pp.first_placed, st));
+        if (ts) {
+            if (counts0)
+                CUDA_TRY(cudaMemcpyAsync(ts->node_count, counts0, sizeof(int32_t) * N * ts->keys, cudaMemcpyDeviceToDevice, st));
+            TRY(ts_prepare(ctx, tp, pod_idx, P, N, true, st));
+        }
         TRY(launch_pipeline<false>(ctx, D, pp, plan.stages, st));
     }
     if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev1, st));
@@ -1976,8 +2247,10 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                                   uint64_t *out_evals, cudaStream_t st, const FirstPassDone *pre = nullptr,
                                   const uint8_t *pod_class = nullptr, const uint64_t *pool_match_host = nullptr,
                                   const acsfit_anti_affinity *aa = nullptr, const acsfit_pod_affinity *pa = nullptr,
-                                  uint64_t present = 0)
+                                  uint64_t present = 0, const acsfit_topology_spread *ts = nullptr)
 {
+    // ts (needs pa): topology spread; every bin pass runs the AA + PA + TS form.  A new bin starts with count 0 and
+    // the minimum is taken as 0 there, so the limits are maxSkew - self throughout: no rises, no reruns.
     // aa: anti-affinity masks of the pods (indexed like req rows); every bin pass runs the AA form, unchained
     // pa (needs aa): pod-affinity masks; every bin pass runs the AA + PA form.  `present`: the signatures already held
     // (by the nodes); it gains those of the pods placed in each pool's bins.  A pool's packing runs again for every
@@ -2012,6 +2285,11 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
         first_placed = fp_;
         evals_save = red_ + 1;
         TRY(or_rows(ctx, pa->pod_self, row_map, Pp, nullptr, red_, &selfs, st));
+    }
+    TsPass tp;
+    if (ts) {
+        TRY(ts_alloc(ctx, ts, Pp, tp));
+        TRY(ts_prepare(ctx, tp, row_map, Pp, 0, false, st));
     }
 
     if (T > 0) CUDA_TRY(cudaMemcpyAsync(unit_dev, unit_host, sizeof(double) * T * D, cudaMemcpyHostToDevice, st));
@@ -2143,6 +2421,12 @@ static acsfit_status fulfill_impl(acsfit_ctx *ctx, const double *req, const int3
                     pp.pod_aff_matches = reinterpret_cast<const unsigned long long *>(pa->pod_matches);
                     pp.first_placed = first_placed;
                     pp.watch = watch & ~fixed;
+                }
+                if (ts) {
+                    pp.ts_key = ts->pod_key;
+                    pp.ts_lim = tp.lim;
+                    pp.ts_matches = reinterpret_cast<const unsigned long long *>(ts->pod_matches);
+                    pp.ts_keys = ts->keys;
                 }
                 if (ctx->timing) CUDA_TRY(cudaEventRecord(ctx->ev0, st));
                 ctx->rec_pool = t;
@@ -3134,13 +3418,55 @@ static acsfit_status zero_aa(acsfit_ctx *ctx, int64_t rows, int64_t N, acsfit_an
     return ACSFIT_OK;
 }
 
-// pa == nullptr: the *_aa form (aa required); otherwise the *_pa form (aa may be NULL)
+// topology spread (include/acsfit.h, acsfit_topology_spread): the *_ts entry points share the *_pa ones'
+// implementation.  rows: request rows, N: nodes (0: fulfill, which reads neither counts nor domains)
+static acsfit_status check_ts_host(acsfit_ctx *ctx, const acsfit_topology_spread *ts, int64_t rows, int64_t N,
+                                   int *flag_dev, cudaStream_t st, const char *what)
+{
+    if (!ts) return fail(ctx, ACSFIT_E_INVALID, "%s: topology-spread arrays missing", what);
+    if (ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: topology spread is not supported in cluster mode", what);
+    if (ts->keys < 0 || ts->keys > ACSFIT_MAX_TS_KEYS)
+        return fail(ctx, ACSFIT_E_INVALID, "%s: %d spread keys, at most %d", what, ts->keys, ACSFIT_MAX_TS_KEYS);
+    if ((rows > 0 && (!ts->pod_key || !ts->pod_skew || !ts->pod_matches)) ||
+        (N > 0 && ts->keys > 0 && (!ts->node_count || !ts->node_domain)) || (N > 0 && ts->keys > 0 && !ts->floor))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: topology-spread field missing", what);
+    for (int k = 0; N > 0 && k < ts->keys; ++k)
+        if (ts->floor[k] < 0) return fail(ctx, ACSFIT_E_INVALID, "%s: floor[%d] = %d is negative", what, k, ts->floor[k]);
+    const int64_t counts = N > 0 ? N * ts->keys : 0;
+    if (rows <= 0 && counts <= 0) return ACSFIT_OK;
+    CUDA_TRY(cudaMemsetAsync(flag_dev, 0, sizeof(int), st));
+    ts_check_kernel<<<grid_for(ctx, std::max(rows, counts), 256), 256, 0, st>>>(
+        ts->pod_key, ts->pod_skew, reinterpret_cast<const unsigned long long *>(ts->pod_matches), rows, ts->keys,
+        ts->node_count, counts, flag_dev);
+    ++ctx->launches;
+    int flag = 0;
+    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    if (flag & 8)
+        return fail(ctx, ACSFIT_E_INVALID, "%s: a pod_key is >= keys, a pod_skew is negative, or a pod_matches names a "
+                    "key >= keys", what);
+    if (flag & 16) return fail(ctx, ACSFIT_E_INVALID, "%s: a node count is negative", what);
+    return ACSFIT_OK;
+}
+
+// zero pod-affinity masks for a topology-spread call without `pa` (rows pods, N nodes), from the arena
+static acsfit_status zero_pa(acsfit_ctx *ctx, int64_t rows, int64_t N, acsfit_pod_affinity *out, cudaStream_t st)
+{
+    TAKE(z, uint64_t, (size_t)3 * rows + (size_t)N);
+    CUDA_TRY(cudaMemsetAsync(z, 0, sizeof(uint64_t) * std::max<size_t>(1, (size_t)3 * rows + (size_t)N), st));
+    *out = {z, z + rows, z + 2 * rows, z + 3 * rows};
+    return ACSFIT_OK;
+}
+
+// pa == nullptr and ts == nullptr: the *_aa form (aa required); otherwise the *_pa / *_ts form (aa, and for *_ts pa,
+// may be NULL)
 static acsfit_status first_fit_nodes_aa_pa(acsfit_ctx *ctx, const double *req, int64_t req_rows, const int32_t *pod_idx,
                                            int64_t P, int D, const double *cap_type, const int32_t *node_type,
                                            double *used_inout, int64_t N, const acsfit_selectors *sel,
                                            const acsfit_anti_affinity *aa, const acsfit_pod_affinity *pa,
                                            int32_t *out_placed, uint64_t *out_decisions, acsfit_stream_t stream,
-                                           const char *what)
+                                           const char *what, const acsfit_topology_spread *ts = nullptr)
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
@@ -3150,8 +3476,9 @@ static acsfit_status first_fit_nodes_aa_pa(acsfit_ctx *ctx, const double *req, i
     if (!pipeline_dims_ok(D))
         return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
     TRY(check_req_aligned(ctx, req, what));
-    if (!pa || aa) TRY(check_aa_host(ctx, aa, req_rows, N, what));
+    if ((!pa && !ts) || aa) TRY(check_aa_host(ctx, aa, req_rows, N, what));
     if (sel) TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, what));
+    if (ts && ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: topology spread is not supported in cluster mode", what);
     reset_stats(ctx);
     // without selectors: class 0 for every row and all-ones node masks, from the arena
     const size_t trivial = sel ? 0 : align_up((size_t)req_rows, 256) + sizeof(uint64_t) * (size_t)N + 512;
@@ -3159,11 +3486,25 @@ static acsfit_status first_fit_nodes_aa_pa(acsfit_ctx *ctx, const double *req, i
     const size_t pa_bytes = !pa ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)(req_rows + N) + 256) +
                                           sizeof(uint64_t) * (size_t)P + sizeof(double) * (size_t)N * D +
                                           sizeof(uint64_t) * 3 * (size_t)N + 2048;
-    TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + trivial + pa_bytes + 1024, st));
+    // topology spread: zero pod-affinity masks without `pa` (and then the pod-affinity scratch), the limits, the
+    // saved counts of a rerun
+    const size_t pa_n = ts && !pa ? (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)(req_rows + N) + 256) +
+                                        sizeof(uint64_t) * (size_t)P + sizeof(double) * (size_t)N * D +
+                                        sizeof(uint64_t) * 3 * (size_t)N + 2048
+                                  : 0;
+    const size_t ts_bytes = !ts ? 0 : pa_n + (pa ? 0 : sizeof(uint64_t) * (size_t)(3 * req_rows + N) + 256) +
+                                          ts_scratch(P) + sizeof(int32_t) * (size_t)N * std::max(0, ts->keys) + 256;
+    TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + trivial + pa_bytes + ts_bytes + 1024, st));
     ctx->arena_off = 0;
     TAKE(flag, int, 1);
     TRY(check_domain(ctx, req, req_rows * D, flag, st, "req"));
     if (pa) TRY(check_pa_host(ctx, pa, req_rows, N, flag, st, what));
+    if (ts) TRY(check_ts_host(ctx, ts, req_rows, N, flag, st, what));
+    acsfit_pod_affinity zero_p;
+    if (ts && !pa) {
+        TRY(zero_pa(ctx, req_rows, N, &zero_p, st));
+        pa = &zero_p;
+    }
     acsfit_anti_affinity zero;
     if (pa && !aa) {
         TRY(zero_aa(ctx, req_rows, N, &zero, st));
@@ -3185,7 +3526,7 @@ static acsfit_status first_fit_nodes_aa_pa(acsfit_ctx *ctx, const double *req, i
     }
     if (P > 0 && N > 0) TRY(build_ranks(ctx, req, req_rows, D, st));
     return first_fit_impl(ctx, req, pod_idx, P, D, cap_type, node_type, used_inout, N, out_placed,
-                          reinterpret_cast<unsigned long long *>(out_decisions), st, pod_class, node_match, aa, pa);
+                          reinterpret_cast<unsigned long long *>(out_decisions), st, pod_class, node_match, aa, pa, ts);
 }
 
 extern "C" acsfit_status acsfit_first_fit_nodes_aa(acsfit_ctx *ctx, const double *req, int64_t req_rows,
@@ -3218,7 +3559,8 @@ static acsfit_status fulfill_pending_aa_pa(acsfit_ctx *ctx, const double *req, i
                                            const acsfit_pod_affinity *pa, uint64_t present, int64_t *out_new_size,
                                            int64_t *out_units_needed, int64_t *out_bins_opened, int32_t *out_acc_pool,
                                            int32_t *out_bin_of, int64_t *out_unaccounted, uint64_t *out_evals,
-                                           acsfit_stream_t stream, const char *what)
+                                           acsfit_stream_t stream, const char *what,
+                                           const acsfit_topology_spread *ts = nullptr)
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
@@ -3231,15 +3573,23 @@ static acsfit_status fulfill_pending_aa_pa(acsfit_ctx *ctx, const double *req, i
     if (!pipeline_dims_ok(D))
         return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
     TRY(check_req_aligned(ctx, req, what));
-    if (!pa || aa) TRY(check_aa_host(ctx, aa, Pp, 0, what));
+    if ((!pa && !ts) || aa) TRY(check_aa_host(ctx, aa, Pp, 0, what));
     if (sel) TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, what));
+    if (ts && ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: topology spread is not supported in cluster mode", what);
     reset_stats(ctx);
-    const size_t pa_bytes = !pa ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)Pp + 256) + sizeof(uint64_t) * (size_t)Pp + 2048;
-    TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + pa_bytes + 1024, st));
+    const size_t pa_bytes = !pa && !ts ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)Pp + 256) + sizeof(uint64_t) * (size_t)Pp + 2048;
+    const size_t ts_bytes = !ts ? 0 : (pa ? 0 : sizeof(uint64_t) * 3 * (size_t)Pp + 256) + ts_scratch(Pp);
+    TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + pa_bytes + ts_bytes + 1024, st));
     ctx->arena_off = 0;
     TAKE(flag, int, 1);
     TRY(check_domain(ctx, req, Pp * D, flag, st, "req"));
     if (pa) TRY(check_pa_host(ctx, pa, Pp, 0, flag, st, what));
+    if (ts) TRY(check_ts_host(ctx, ts, Pp, 0, flag, st, what));
+    acsfit_pod_affinity zero_p;
+    if (ts && !pa) {
+        TRY(zero_pa(ctx, Pp, 0, &zero_p, st));
+        pa = &zero_p;
+    }
     acsfit_anti_affinity zero;
     if (pa && !aa) {
         TRY(zero_aa(ctx, Pp, 0, &zero, st));
@@ -3250,7 +3600,7 @@ static acsfit_status fulfill_pending_aa_pa(acsfit_ctx *ctx, const double *req, i
     return fulfill_impl(ctx, req, nullptr, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
                         over_provision, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
                         out_unaccounted, out_evals, st, nullptr, sel ? sel->pod_class : nullptr,
-                        sel ? sel->pool_match_ordered : nullptr, aa, pa, present);
+                        sel ? sel->pool_match_ordered : nullptr, aa, pa, present, ts);
 }
 
 extern "C" acsfit_status acsfit_fulfill_pending_aa(acsfit_ctx *ctx, const double *req, int64_t Pp,
@@ -3283,6 +3633,36 @@ extern "C" acsfit_status acsfit_fulfill_pending_pa(acsfit_ctx *ctx, const double
     return fulfill_pending_aa_pa(ctx, req, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
                                  over_provision, sel, aa, pa, present, out_new_size, out_units_needed, out_bins_opened,
                                  out_acc_pool, out_bin_of, out_unaccounted, out_evals, stream, "fulfill_pending_pa");
+}
+
+extern "C" acsfit_status acsfit_first_fit_nodes_ts(acsfit_ctx *ctx, const double *req, int64_t req_rows,
+                                                   const int32_t *pod_idx, int64_t P, int D, const double *cap_type,
+                                                   const int32_t *node_type, double *used_inout, int64_t N,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, const acsfit_topology_spread *ts,
+                                                   int32_t *out_placed, uint64_t *out_decisions, acsfit_stream_t stream)
+{
+    if (ctx && !ts) return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_ts: topology-spread arrays missing");
+    return first_fit_nodes_aa_pa(ctx, req, req_rows, pod_idx, P, D, cap_type, node_type, used_inout, N, sel, aa, pa,
+                                 out_placed, out_decisions, stream, "first_fit_nodes_ts", ts);
+}
+
+extern "C" acsfit_status acsfit_fulfill_pending_ts(acsfit_ctx *ctx, const double *req, int64_t Pp,
+                                                   int64_t num_listed, int D, const double *unit,
+                                                   const int32_t *pool_actual, const int32_t *pool_max,
+                                                   const uint8_t *pool_ignored, int T, int64_t over_provision,
+                                                   const acsfit_selectors *sel, const acsfit_anti_affinity *aa,
+                                                   const acsfit_pod_affinity *pa, uint64_t present,
+                                                   const acsfit_topology_spread *ts, int64_t *out_new_size,
+                                                   int64_t *out_units_needed, int64_t *out_bins_opened,
+                                                   int32_t *out_acc_pool, int32_t *out_bin_of,
+                                                   int64_t *out_unaccounted, uint64_t *out_evals,
+                                                   acsfit_stream_t stream)
+{
+    if (ctx && !ts) return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_ts: topology-spread arrays missing");
+    return fulfill_pending_aa_pa(ctx, req, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                                 over_provision, sel, aa, pa, present, out_new_size, out_units_needed, out_bins_opened,
+                                 out_acc_pool, out_bin_of, out_unaccounted, out_evals, stream, "fulfill_pending_ts", ts);
 }
 
 // ---------------------------------------------------------------------------------------------

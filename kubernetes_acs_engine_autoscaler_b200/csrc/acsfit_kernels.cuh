@@ -170,6 +170,22 @@ struct PipelineParams {
     unsigned long long *node_has;               // [N] in/out (node pass)
     unsigned long long *first_placed;           // [64]: atomicMin of the position of each placed pod that matches a watched signature
     unsigned long long watch;                   // signatures whose first placement is recorded (0: none, nothing recorded)
+    // hostname topology spread (TS instantiations, built on the PA form; appended).  A pod with a key (ts_key != 0xFF)
+    // may take a node (bin) only when the node's count of that key is <= the pod's limit ts_lim (maxSkew - self +
+    // the key's minimum at the pod's position, indexed like pod_need); the taker adds 1 to the node's count of every
+    // key of its ts_matches.  Node passes read and write ts_count (key-major, row stride ts_stride); bins start at 0
+    // and are not written back.  Node passes also report, per key k with ts_target[k] != INT_MAX, every take that
+    // brings a domain of k (ts_domain) to exactly ts_target[k]: ts_reached[k] += 1, ts_rise_pos[k] = max position.
+    const uint8_t *ts_key;                      // [req rows] the pod's key, 0xFF none
+    const int32_t *ts_lim;                      // [positions]
+    const unsigned long long *ts_matches;       // [req rows] keys whose selector selects the pod
+    int32_t *ts_count;                          // [ts_keys][ts_stride] in/out (node pass)
+    const unsigned long long *ts_domain;        // [N] keys each node is a domain of (node pass)
+    const int *ts_target;                       // [64] (node pass)
+    int *ts_reached;                            // [64] (node pass)
+    unsigned long long *ts_rise_pos;            // [64] (node pass)
+    int64_t ts_stride;
+    int ts_keys;
 };
 
 __device__ __forceinline__ int ld_acquire(const int *p)
@@ -244,10 +260,12 @@ __device__ __forceinline__ void load_row(double (&r)[D], const double *src)
 // dynamic shared memory layout (doubles first for alignment).
 // nodes mode keeps three [D][Tn] arrays: scan thresholds, used (the mutable state) and capacity;
 // bins mode keeps one: the remaining capacity IS the threshold (finite values, Lemma B).
-template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false, bool AA = false, bool PA = false>
+template <int D, bool BINS, int NT, bool PRUNE = false, int RW = 0, bool SEL = false, bool AA = false, bool PA = false,
+          bool TS = false>
 struct PipelineSmem {
     static constexpr int NW = NT / 32;  // warps per stage CTA == resolver warps
-    static __host__ __device__ size_t bytes(int Tn)
+    // TS: the counts are sized by the call's key count, not by 64
+    static __host__ __device__ size_t bytes(int Tn, int ts_keys = 0)
     {
         return sizeof(double) * ((size_t)kTile * D + (size_t)(BINS ? 1 : 3) * D * Tn + (size_t)NW * 36 * D /*batch rows*/ + (PRUNE ? (size_t)(NW + 1) * D : 0) /*warp bounds + stage bound*/)
                + sizeof(unsigned) * (kTile /*cand*/ + kTile / 32 /*hit*/ + kTile / 32 /*alive*/ + NW /*opened*/ +
@@ -258,7 +276,9 @@ struct PipelineSmem {
                + (SEL ? sizeof(unsigned long long) * (size_t)Tn /*node masks*/ + kTile /*pod classes*/ + (size_t)NW * 36 /*batch classes*/ : 0)
                + (AA ? sizeof(unsigned long long) * 2 * ((size_t)Tn /*node carries / matches*/ + kTile /*pod masks*/ + (size_t)NW * 36 /*batch masks*/) : 0)
                + (PA ? sizeof(unsigned long long) * ((size_t)Tn /*node has*/ + 2 * ((size_t)kTile /*pod need / matches*/ + (size_t)NW * 36 /*batch*/)) : 0)
-               + (BINS && RW > 0 ? sizeof(double) * (size_t)D * (1 /*smallest request*/ + kRankStaged /*staged rank tables*/) : 0);
+               + (BINS && RW > 0 ? sizeof(double) * (size_t)D * (1 /*smallest request*/ + kRankStaged /*staged rank tables*/) : 0)
+               + (TS ? sizeof(unsigned long long) * (2 * ((size_t)kTile /*pod key+limit / matches*/ + (size_t)NW * 36 /*batch*/) + (size_t)Tn /*node domains*/)
+                           + sizeof(int) * (64 /*targets*/ + (size_t)ts_keys * Tn /*counts*/) : 0);
     }
 };
 
@@ -311,13 +331,22 @@ __device__ __forceinline__ unsigned wait_entry(const volatile unsigned *slot, in
 // which stay resource (plus class) only and hence a superset filter, and is evaluated in the resolver alone, whose
 // chain sees every node's state exactly as the sequential loop does.  The need itself is fixed for the pass (the host
 // applies the bootstrap exception through flip positions, see acsfit.cu).
-template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false, bool AA = false, bool PA = false>
+//
+// TS (on top of the PA form): hostname topology spread.  A pod with a key may take a node (bin) only while the node's
+// count of that key stays within the pod's limit; the taker adds 1 to its node's count of every key the pod matches.
+// Counts only grow, but in a node pass the limit (which carries the key's minimum over its domains) is fixed per
+// position by the host and rises where the minimum does, so the test is not monotone: like PA it lives in the
+// resolver alone, and the scan, bounds, pruning and retirement stay resource (plus class) only.  A new bin starts
+// with count 0 and admits any pod (limit >= 0), so the untouched-bin shortcut stays exact.  Node passes report the
+// takes that bring a watched key's domain to its target count (the next rise of its minimum, see acsfit.cu).
+template <int D, bool BINS, int NT, bool PRUNE, int RW, bool SEL = false, bool AA = false, bool PA = false, bool TS = false>
 __global__ void __launch_bounds__(NT, D <= 4 ? 2 : 1)
 firstfit_pipeline_kernel(const PipelineParams p)
 {
     static_assert(!(SEL && BINS), "selectors apply to node passes only");
     static_assert(!AA || BINS || SEL, "the anti-affinity node pass builds on the selector form");
     static_assert(!PA || AA, "the pod-affinity form builds on the anti-affinity form");
+    static_assert(!TS || PA, "the topology-spread form builds on the pod-affinity form");
     constexpr int K = nodes_per_thread(D, RW);  // RW: 32-bit words of a packed-rank row, 0 = float64 scan
     constexpr int NW = NT / 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -367,6 +396,15 @@ firstfit_pipeline_kernel(const PipelineParams p)
     // bins with the packed-rank scan: the smallest request of each dimension and the staged rank tables
     double *minreq_s = reinterpret_cast<double *>(PA ? bm_s + NW * 36 : AA ? bx_s + NW * 36 : nm_s);  // [D]
     double *rt_s = minreq_s + D;                                                 // [D][kRankStaged]
+    // TS: key + limit (+ slot, in the batch) and key matches of the tile's compacted pods and of each resolver batch,
+    // domain masks, targets and counts ([key][Tn]) of the stage's nodes
+    unsigned long long *tk_s = reinterpret_cast<unsigned long long *>(minreq_s + (BINS && RW > 0 ? D * (1 + kRankStaged) : 0));  // [kTile]
+    unsigned long long *tm_s = tk_s + kTile;       // [kTile]
+    unsigned long long *bk_s = tm_s + kTile;       // [NW][36]
+    unsigned long long *bt_s = bk_s + NW * 36;     // [NW][36]
+    unsigned long long *nd_s = bt_s + NW * 36;     // [Tn]
+    int *tgt_s = reinterpret_cast<int *>(nd_s + Tn);  // [64]
+    int *cnt_s = tgt_s + 64;                          // [ts_keys][Tn]
 
     const int tid = threadIdx.x;
     const int lane = tid & 31;
@@ -431,6 +469,14 @@ firstfit_pipeline_kernel(const PipelineParams p)
         }
     if constexpr (PA)
         for (int n = tid; n < Tn; n += NT) nh_s[n] = !BINS && n < n_valid ? p.node_has[stage_lo + n] : 0ull;
+    if constexpr (TS) {  // bins (and padding nodes) start with count 0 and are nobody's domain
+        for (int n = tid; n < Tn; n += NT) nd_s[n] = !BINS && n < n_valid ? p.ts_domain[stage_lo + n] : 0ull;
+        for (int i = tid; i < p.ts_keys * Tn; i += NT) {
+            const int k = i / Tn, n = i - k * Tn;
+            cnt_s[i] = !BINS && n < n_valid ? p.ts_count[(size_t)k * p.ts_stride + stage_lo + n] : 0;
+        }
+        if (tid < 64) tgt_s[tid] = !BINS && tid < p.ts_keys ? p.ts_target[tid] : INT_MAX;
+    }
     // Bin retirement (RW > 0).  The rank tables are built over every request row of the call, a superset of the pass's
     // pods, so sorted[d][0] is a lower bound of every request of the pass in dimension d.  A bin with S[d] < that
     // bound in some d can take no pod of the pass now, and S only shrinks: it is dead for good.  Without rank tables
@@ -513,6 +559,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
     unsigned pre_cls = 0;  // SEL: the entry's selector class
     unsigned long long pre_c = 0ull, pre_x = 0ull;  // AA: the entry's carries / matches
     unsigned long long pre_n = 0ull, pre_m = 0ull;  // PA: the entry's need / signature matches
+    unsigned long long pre_k = 0ull, pre_t = 0ull;  // TS: the entry's key << 32 | limit, and key matches
     auto prefetch_row = [&](int tile) {
         const int64_t j = (int64_t)(p.tile_lo + tile) * kTile + tid;
         if (tid < kTile && tile < p.num_tiles && j < p.M) {
@@ -537,6 +584,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
             if constexpr (PA) {
                 pre_n = __ldg(p.pod_need + (BINS ? (int64_t)__ldg(p.pod_idx + j) : j));
                 pre_m = __ldg(p.pod_aff_matches + row);
+            }
+            if constexpr (TS) {
+                const int lim = __ldg(p.ts_lim + (BINS ? (int64_t)__ldg(p.pod_idx + j) : j));
+                pre_k = ((unsigned long long)__ldg(p.ts_key + row) << 32) | (unsigned)lim;
+                pre_t = __ldg(p.ts_matches + row);
             }
         }
     };
@@ -663,6 +715,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
             if constexpr (PA) {
                 pn_s[pos] = pre_n;
                 pm_s[pos] = pre_m;
+            }
+            if constexpr (TS) {
+                tk_s[pos] = pre_k;
+                tm_s[pos] = pre_t;
             }
         }
         prefetch_row(tile + 1);
@@ -891,6 +947,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
                 }
                 unsigned long long my_nh = 0ull;  // PA: this lane's node's has mask
                 if constexpr (PA) my_nh = n < Tn ? nh_s[n] : 0ull;
+                unsigned long long my_nd = 0ull;  // TS: the keys this lane's node is a domain of (node pass)
+                if constexpr (TS) my_nd = n < Tn ? nd_s[n] : 0ull;
+                // TS: this lane's column of the counts.  A lane past the stage's nodes (stages narrower than a warp)
+                // fits no entry and so never takes: it reads column 0, which keeps every access inside the array.
+                const int my_cn = n < Tn ? n : 0;
 
                 unsigned my_takes = 0;  // pods this lane's node / bin took in this tile
                 const volatile unsigned *in_q = BINS ? (chain_below ? queue + (size_t)(31 - __clz(chain_below)) * (kTile + 1) : hitlist)
@@ -971,6 +1032,7 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     unsigned char *bcls = bcls_s + warp * 36;  // SEL: class of each dense entry (+4 padding entries)
                     unsigned long long *bc = bc_s + warp * 36, *bx = bx_s + warp * 36;  // AA: masks of each dense entry
                     unsigned long long *bn = bn_s + warp * 36, *bm = bm_s + warp * 36;  // PA: need / matches of each dense entry
+                    unsigned long long *bk = bk_s + warp * 36, *bt = bt_s + warp * 36;  // TS: key + limit + slot / matches
                     if (poss) {
 #pragma unroll
                         for (int d = 0; d < D; d += 2)
@@ -983,6 +1045,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         if constexpr (PA) {
                             bn[my_rank] = pn_s[q_l];
                             bm[my_rank] = pm_s[q_l];
+                        }
+                        if constexpr (TS) {
+                            bk[my_rank] = tk_s[q_l] | ((unsigned long long)s_l << 40);
+                            bt[my_rank] = tm_s[q_l];
                         }
                     }
                     fnd[lane] = 0xFF;  // "nobody took dense entry `lane`" until a taker says otherwise
@@ -1000,6 +1066,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         if constexpr (PA) {
                             bn[n_poss + lane] = 0ull;
                             bm[n_poss + lane] = 0ull;
+                        }
+                        if constexpr (TS) {
+                            bk[n_poss + lane] = 0xFFull << 32;  // no key
+                            bt[n_poss + lane] = 0ull;
                         }
                     }
                     __syncwarp();
@@ -1020,6 +1090,13 @@ firstfit_pipeline_kernel(const PipelineParams p)
                     if constexpr (PA) {
                         en = bn[0];
                         em = bm[0];
+                    }
+                    // TS: the entry's key + limit + slot and key matches, loaded one entry ahead; the count itself is
+                    // read after the previous entry's take (this lane alone writes its node's counts)
+                    unsigned long long ek = 0ull, et = 0ull;
+                    if constexpr (TS) {
+                        ek = bk[0];
+                        et = bt[0];
                     }
                     const long long t_l0 = tracing ? clock64() : 0;
                     if (tracing) n_iter += (unsigned)n_poss;
@@ -1062,10 +1139,19 @@ firstfit_pipeline_kernel(const PipelineParams p)
                             en_next = bn[k + 1];
                             em_next = bm[k + 1];
                         }
+                        unsigned long long ek_next = 0ull, et_next = 0ull;
+                        if constexpr (TS) {
+                            ek_next = bk[k + 1];
+                            et_next = bt[k + 1];
+                        }
                         bool ok = fits(S, r);
                         if constexpr (SEL) ok = ok & mt;
                         if constexpr (AA) ok = ok & (((ec & my_nx) | (ex & my_nc)) == 0ull);
                         if constexpr (PA) ok = ok & (en == 0ull || (en & my_nh) != 0ull);
+                        if constexpr (TS) {
+                            const unsigned key = (unsigned)(ek >> 32) & 0xFFu;
+                            ok = ok & (key == 0xFFu || cnt_s[key * Tn + my_cn] <= (int)(unsigned)ek);
+                        }
                         // the vote-to-vote path: ballot -> "no fitting lane before me" -> predicated update of S -> next
                         // test.  No branch on it (at the frontier nearly every entry is taken) and no mask arithmetic
                         // beyond one and + compare.
@@ -1078,6 +1164,20 @@ firstfit_pipeline_kernel(const PipelineParams p)
                             mask_take(my_nx, ex, loses);
                         }
                         if constexpr (PA) mask_take(my_nh, em, loses);
+                        if constexpr (TS) {
+                            if (!loses && et) {  // the taker counts the pod on its node under every key it matches
+                                const int64_t jj = (int64_t)(p.tile_lo + tile) * kTile + (int64_t)((ek >> 40) & 0xFFu);
+                                for (unsigned long long w = et; w; w &= w - 1) {
+                                    const int b = __ffsll((long long)w) - 1;
+                                    const int c = cnt_s[b * Tn + my_cn] + 1;
+                                    cnt_s[b * Tn + my_cn] = c;
+                                    if (!BINS && c == tgt_s[b] && ((my_nd >> b) & 1ull)) {  // a domain reached the target
+                                        atomicAdd(p.ts_reached + b, 1);
+                                        atomicMax(p.ts_rise_pos + b, (unsigned long long)jj);
+                                    }
+                                }
+                            }
+                        }
                         note_take(fnd_sa + (unsigned)k, (unsigned)lane, loses);  // off the chain: who took entry k
                         my_takes += loses ? 0u : 1u;
 #pragma unroll
@@ -1090,6 +1190,10 @@ firstfit_pipeline_kernel(const PipelineParams p)
                         if constexpr (PA) {
                             en = en_next;
                             em = em_next;
+                        }
+                        if constexpr (TS) {
+                            ek = ek_next;
+                            et = et_next;
                         }
                     }
                     __syncwarp();
@@ -1253,6 +1357,11 @@ firstfit_pipeline_kernel(const PipelineParams p)
             }
         if constexpr (PA)
             for (int n = tid; n < n_valid; n += NT) p.node_has[stage_lo + n] = nh_s[n];
+        if constexpr (TS)
+            for (int i = tid; i < p.ts_keys * Tn; i += NT) {
+                const int k = i / Tn, n = i - k * Tn;
+                if (n < n_valid) p.ts_count[(size_t)k * p.ts_stride + stage_lo + n] = cnt_s[i];
+            }
     }
     if (BINS && lane == 0 && my_evals) atomicAdd(p.evals, my_evals);  // every warp credits its own placements
     if (tid == 0) {

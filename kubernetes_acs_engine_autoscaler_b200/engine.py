@@ -527,6 +527,82 @@ class Engine(object):
                 "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
                 "evals": int(evals.value)}
 
+    # ------------------------------------------------------------------ topology spread (include/acsfit.h)
+    def last_spread_rises(self):
+        """test hook: the (key, position) rises the last topology-spread call fixed, one per pass it ran again."""
+        n = ctypes.c_int64(0)
+        self._check(self._lib.acsfit_last_spread_rises(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p), None))
+        out = np.zeros(2 * n.value, dtype=np.int64)
+        self._check(self._lib.acsfit_last_spread_rises(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p),
+                                                       _ptr(out)))
+        return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(n.value)]
+
+    @staticmethod
+    def _spread(keys, pod_key, pod_skew, pod_matches, node_count=None, node_domain=None, floor=None):
+        floor = np.ascontiguousarray(np.zeros(0, np.int32) if floor is None else floor, dtype=np.int32)
+        keep = [pod_key, pod_skew, pod_matches, node_count, node_domain, floor]
+        ts = _native.TopologySpread(*[None if a is None else _ptr(a).value for a in keep[:5]], _ptr(floor).value,
+                                    int(keys))
+        return ts, keep
+
+    def first_fit_nodes_ts(self, req, pod_idx, cap_type, node_type, used, keys, pod_key, pod_skew, pod_matches,
+                           node_count, node_domain, floor, pa=None, aa=None, pod_class=None, node_match=None, classes=1):
+        """first_fit_nodes with hostname topology spread: pod_key uint8 [req rows], pod_skew int32 [req rows],
+        pod_matches uint64 [req rows] (stored as int64), node_count int32 [keys, N] and node_domain uint64 [N] device,
+        floor int32 [keys] host; node_count is updated in place like `used`.  `pa` (pod_requires, pod_self,
+        pod_matches, node_has) and `aa` (pod_carries, pod_matches, node_carries, node_matches) device tuples or None;
+        pod_class / node_match (both or neither) as in first_fit_nodes_aa."""
+        rows, D = req.shape
+        P = rows if pod_idx is None else pod_idx.shape[0]
+        N = used.shape[0]
+        placed = self.empty((P,), torch.int32)
+        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
+        sel, keep_s = (None, None) if pod_class is None else \
+            self._selectors(classes, pod_class=pod_class, node_match=node_match)
+        a, keep_a = (None, None) if aa is None else self._anti_affinity(*aa)
+        p = None if pa is None else _native.PodAffinity(*[_ptr(t).value for t in pa])
+        ts, keep_t = self._spread(keys, pod_key, pod_skew, pod_matches, node_count, node_domain, floor)
+        ref = lambda s: None if s is None else ctypes.cast(ctypes.byref(s), ctypes.c_void_p)  # noqa: E731
+        self._check(self._lib.acsfit_first_fit_nodes_ts(
+            self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
+            ref(sel), ref(a), ref(p), ref(ts), _ptr(placed), _ptr(decisions), self._stream()))
+        return placed, decisions
+
+    def fulfill_pending_ts(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision, keys,
+                           pod_key, pod_skew, pod_matches, pa=None, present=0, aa=None, pod_class=None,
+                           pool_match=None, classes=1):
+        """fulfill_pending with hostname topology spread in the bins: pod_key / pod_skew / pod_matches [Pp] device as
+        in first_fit_nodes_ts.  `pa` (pod_requires, pod_self, pod_matches) and `aa` (pod_carries, pod_matches) device
+        tuples or None; `present` and pod_class / pool_match as in fulfill_pending_pa."""
+        Pp, D = req.shape
+        unit = _np(unit, np.float64).reshape(-1, D)
+        T = unit.shape[0]
+        pool_actual = _np(pool_actual, np.int32)
+        pool_max = _np(pool_max, np.int32)
+        pool_ignored = _np(pool_ignored, np.uint8)
+        new_size = np.zeros(T, dtype=np.int64)
+        units_needed = np.zeros(T, dtype=np.int64)
+        bins_opened = np.zeros(T, dtype=np.int64)
+        acc_pool = self.empty((Pp,), torch.int32)
+        bin_of = self.empty((Pp,), torch.int32)
+        unacc = ctypes.c_int64(0)
+        evals = ctypes.c_uint64(0)
+        sel, keep_s = (None, None) if pod_class is None else \
+            self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
+        a, keep_a = (None, None) if aa is None else self._anti_affinity(*aa)
+        p = None if pa is None else _native.PodAffinity(*[_ptr(t).value for t in pa], None)
+        ts, keep_t = self._spread(keys, pod_key, pod_skew, pod_matches)
+        ref = lambda s: None if s is None else ctypes.cast(ctypes.byref(s), ctypes.c_void_p)  # noqa: E731
+        self._check(self._lib.acsfit_fulfill_pending_ts(
+            self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
+            _ptr(pool_ignored), T, int(over_provision), ref(sel), ref(a), ref(p), int(present) & 0xFFFFFFFFFFFFFFFF,
+            ref(ts), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(bin_of),
+            ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p), ctypes.cast(ctypes.byref(evals), ctypes.c_void_p),
+            self._stream()))
+        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
+                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
+                "evals": int(evals.value)}
+
     # ------------------------------------------------------------------ pod affinity (include/acsfit.h)
     def first_fit_nodes_pa(self, req, pod_idx, cap_type, node_type, used, pod_requires, pod_self, pod_matches, node_has,
                            pod_carries=None, pod_matches_aa=None, node_carries=None, node_matches=None, pod_class=None,

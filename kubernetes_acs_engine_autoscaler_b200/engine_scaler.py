@@ -23,7 +23,8 @@ class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                  deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
                  selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False,
-                 anti_affinity_node_states=False, pod_affinity=False, pod_affinity_node_states=False):
+                 anti_affinity_node_states=False, pod_affinity=False, pod_affinity_node_states=False,
+                 topology_spread=False):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
@@ -34,6 +35,7 @@ class EngineScaler(Scaler):
         self.anti_affinity_node_states = anti_affinity_node_states
         self.pod_affinity = pod_affinity
         self.pod_affinity_node_states = pod_affinity_node_states
+        self.topology_spread = topology_spread
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)

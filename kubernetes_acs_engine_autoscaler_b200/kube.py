@@ -195,6 +195,79 @@ def affinity_term_selects(term, namespace, labels):
     return selector is not None and namespace in namespaces and selector_matches(selector, labels)
 
 
+# topology spread: the values Kubernetes validation accepts
+WHEN_UNSATISFIABLE = ('DoNotSchedule', 'ScheduleAnyway')
+NODE_INCLUSION_POLICIES = ('Honor', 'Ignore')
+
+
+class SpreadConstraint(tuple):
+    """the honoured topology spread constraint of a pod: (max_skew, selector, min_domains, honor_affinity,
+    honor_taints).  `selector` is the canonical label_selector with the matchLabelKeys requirements added, or None
+    (a null labelSelector selects no pod); min_domains defaults to 1; honor_affinity / honor_taints are the
+    nodeAffinityPolicy (default Honor) and nodeTaintsPolicy (default Ignore) as booleans."""
+    __slots__ = ()
+
+    max_skew = property(lambda self: self[0])
+    selector = property(lambda self: self[1])
+    min_domains = property(lambda self: self[2])
+    honor_affinity = property(lambda self: self[3])
+    honor_taints = property(lambda self: self[4])
+
+
+def _selector_keys(selector):
+    """the label keys a raw labelSelector names (matchLabels and matchExpressions)"""
+    keys = set((selector.get('matchLabels') or {}).keys())
+    keys.update(e.get('key') for e in selector.get('matchExpressions') or ())
+    return keys
+
+
+def topology_spread_constraint(constraints, labels, owner):
+    """the constraint of spec.topologySpreadConstraints that this project honours, as a SpreadConstraint, or None:
+    the one with topologyKey kubernetes.io/hostname and whenUnsatisfiable DoNotSchedule (validation allows one).
+    Every entry is validated as Kubernetes validates it, and ValueError names the owner when one is malformed:
+    maxSkew an integer >= 1, whenUnsatisfiable one of WHEN_UNSATISFIABLE, a non-empty topologyKey, no duplicate
+    (topologyKey, whenUnsatisfiable), minDomains >= 1 and only with DoNotSchedule, matchLabelKeys neither without a
+    labelSelector nor naming a key the labelSelector names, each policy one of NODE_INCLUSION_POLICIES.  A key of
+    matchLabelKeys adds `key In [the pod's value]` to the selector; a key the pod lacks (in `labels`) adds nothing."""
+    what = 'spec.topologySpreadConstraints'
+    honoured, seen = None, set()
+    for c in _entries(constraints, what, owner):
+        skew, when, topology = c.get('maxSkew'), c.get('whenUnsatisfiable'), c.get('topologyKey')
+        if type(skew) is not int or skew < 1:
+            raise ValueError("malformed %s entry of %s: maxSkew %r (an integer >= 1)" % (what, owner, skew))
+        if when not in WHEN_UNSATISFIABLE:
+            raise ValueError("malformed %s entry of %s: whenUnsatisfiable %r" % (what, owner, when))
+        if not isinstance(topology, str) or not topology:
+            raise ValueError("malformed %s entry of %s: topologyKey %r" % (what, owner, topology))
+        if (topology, when) in seen:
+            raise ValueError("malformed %s of %s: duplicate (topologyKey, whenUnsatisfiable) %r"
+                             % (what, owner, (topology, when)))
+        seen.add((topology, when))
+        min_domains = c.get('minDomains')
+        if min_domains is not None and (type(min_domains) is not int or min_domains < 1 or when != 'DoNotSchedule'):
+            raise ValueError("malformed %s entry of %s: minDomains %r (an integer >= 1, with DoNotSchedule only)"
+                             % (what, owner, min_domains))
+        policies = []
+        for field, default in (('nodeAffinityPolicy', 'Honor'), ('nodeTaintsPolicy', 'Ignore')):
+            value = c.get(field)
+            if value is not None and value not in NODE_INCLUSION_POLICIES:
+                raise ValueError("malformed %s entry of %s: %s %r" % (what, owner, field, value))
+            policies.append((default if value is None else value) == 'Honor')
+        raw = c.get('labelSelector')
+        selector = None if raw is None else label_selector(raw, owner, what + '.labelSelector')
+        keys = _str_list(c.get('matchLabelKeys') or [], what + '.matchLabelKeys', owner)
+        if keys and (raw is None or set(keys) & _selector_keys(raw)):
+            raise ValueError("malformed %s entry of %s: matchLabelKeys %r without a labelSelector or naming one of "
+                             "its keys" % (what, owner, keys))
+        if topology != HOSTNAME_TOPOLOGY_KEY or when != 'DoNotSchedule':
+            continue
+        if selector is not None and keys:
+            extra = [(k, 'In', (labels[k],)) for k in keys if k in labels]
+            selector = (selector[0], tuple(sorted(set(selector[1] + tuple(extra)))))
+        honoured = SpreadConstraint((skew, selector, 1 if min_domains is None else min_domains, *policies))
+    return honoured
+
+
 # required node affinity: the operators of a NodeSelectorRequirement, and the one field a matchFields entry may name
 NODE_SELECTOR_OPERATORS = ('In', 'NotIn', 'Exists', 'DoesNotExist', 'Gt', 'Lt')
 NODE_NAME_FIELD = 'metadata.name'
@@ -457,6 +530,13 @@ class KubePod(object):
     def affinity_terms(self):
         """the honoured required pod affinity terms (kube.affinity_terms); read on use, like tolerations."""
         return affinity_terms(self.original.obj['spec'].get('affinity'), self.namespace, 'pod %s' % self)
+
+    @property
+    def topology_spread(self):
+        """the honoured hostname topology spread constraint (kube.topology_spread_constraint; None when there is none);
+        read on use, like tolerations."""
+        return topology_spread_constraint(self.original.obj['spec'].get('topologySpreadConstraints'), self.labels,
+                                          'pod %s' % self)
 
     @property
     def node_affinity(self):

@@ -80,6 +80,8 @@ class Scaler(object):
         # with pod affinity: POD_PENDING only when some pod to schedule could land on the node given its required pod
         # affinity (Cluster(pod_affinity_node_states=...))
         self.pod_affinity_node_states = False
+        # hostname topology spread (DoNotSchedule) in the bins of fulfill_pending (Cluster(topology_spread=...))
+        self.topology_spread = False
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -139,9 +141,10 @@ class Scaler(object):
                                                 affinity=self.node_affinity)
         anti_affinity = snapshot.anti_affinity(unique) if self.pod_anti_affinity else None
         pod_affinity = snapshot.pod_affinity(unique) if self.pod_affinity else None
+        topology_spread = snapshot.topology_spread(unique) if self.topology_spread else None
         res = snapshot.fulfill(unique, len(pods), ordered_pools, self.ignored_pool_names, self.over_provision,
                                classes=classes, anti_affinity=anti_affinity, pod_affinity=pod_affinity,
-                               affinity_present=affinity_present)
+                               affinity_present=affinity_present, topology_spread=topology_spread)
 
         new_pool_sizes, current_pool_sizes = {}, {}
         unaccounted = len(pods)

@@ -655,6 +655,134 @@ def _pod_affinity_masks(pods, running, run_idx):
 
 
 # ------------------------------------------------------------------------------------------------
+# hostname topology spread: keys, counts and domains (include/acsfit.h, acsfit_topology_spread)
+# ------------------------------------------------------------------------------------------------
+MAX_TS_KEYS = 64
+NO_SPREAD_KEY = 0xFF
+INT32_MAX = 2 ** 31 - 1
+
+
+class TopologySpread(object):
+    """pod_key uint8[P] (the pod's key, NO_SPREAD_KEY without a constraint), pod_skew int32[P] (maxSkew - 1 when the
+    pod's own selector selects it, else maxSkew), pod_matches uint64[P] (the keys whose selector selects the pod),
+    node_count int32[keys, N] (the selected pods on each node), node_domain uint64[N] (the keys each node is a domain
+    of), floor int32[keys] (the smallest count over the key's domains outside the node list, INT32_MAX without one, 0
+    when the key has fewer domains in all than its minDomains) and the keys: (namespace, selector, domain set,
+    minDomains) tuples, bit k = keys[k]."""
+
+    def __init__(self, pod_key, pod_skew, pod_matches, node_count, node_domain, floor, keys):
+        self.pod_key = pod_key
+        self.pod_skew = pod_skew
+        self.pod_matches = pod_matches
+        self.node_count = node_count
+        self.node_domain = node_domain
+        self.floor = floor
+        self.keys = keys
+
+    @property
+    def trivial(self):
+        """no pod of this call has a constraint: the calls without topology spread give the same result"""
+        return not self.keys
+
+
+def _spread_domains(pods, constraints, all_nodes):
+    """(domain key per pod with a constraint, {domain key: bool[len(all_nodes)]}): the nodes counted for each pod's
+    minimum.  nodeAffinityPolicy Honor: the pod's nodeSelector and required node affinity admit the node; nodeTaintsPolicy
+    Honor: the pod tolerates its blocking taints.  Each distinct requirement is evaluated once per node projection."""
+    spec_of, specs = {}, {}
+    for i, c in constraints:
+        pod = pods[i]
+        items = tuple(sorted(pod.selectors.items())) if c.honor_affinity and pod.selectors else ()
+        terms = pod.node_affinity if c.honor_affinity else None
+        tolerations = pod.tolerations if c.honor_taints else None
+        key = (items, terms, None if tolerations is None else _toleration_items(tolerations))
+        spec_of[i] = key
+        specs.setdefault(key, (items, tolerations, terms))
+    if not specs:
+        return spec_of, {}
+    if not all_nodes:
+        return spec_of, {key: np.zeros(0, dtype=bool) for key in specs}
+    taints = any(t is not None for _, t, _ in specs.values())
+    distinct = [(items, t, terms) for items, t, terms in specs.values()]
+    proj = _projection(all_nodes, distinct, taints)
+    domains = {}
+    for key, (items, tolerations, terms) in specs.items():
+        match = proj.selector(items)
+        if terms is not None:
+            match &= proj.affinity(terms)
+        if tolerations is not None:
+            match &= proj.tolerated(tolerations)
+        domains[key] = match[proj.group]
+    return spec_of, domains
+
+
+def topology_spread(pods, nodes=(), running_pods=(), other_nodes=()):
+    """the topology-spread arrays of the pods to place (`pods`) over the agent nodes `nodes`.  `other_nodes` are the
+    nodes of the listing outside them (the master): they cannot take a pod here but they are domains, so their counts
+    go into `floor`.  The pods of `running_pods` on a node count on it, matched by node name as the occupancy count
+    matches them.  A key is a distinct (namespace, selector with the matchLabelKeys values, domain set, minDomains) of
+    the pods' honoured constraints (KubePod.topology_spread), numbered in first-occurrence order; ValueError above 64.
+    Each selector is evaluated once per distinct (namespace, label values it reads) projection of the pods, and each
+    domain requirement once per node projection; nothing of size pods x nodes is built."""
+    pods, nodes, other, running = list(pods), list(nodes), list(other_nodes), list(running_pods)
+    P, N = len(pods), len(nodes)
+    constraints = [(i, c) for i, c in ((i, p.topology_spread) for i, p in enumerate(pods)) if c is not None]
+    pod_key = np.full(P, NO_SPREAD_KEY, dtype=np.uint8)
+    pod_skew = np.zeros(P, dtype=np.int32)
+    if not constraints:
+        return TopologySpread(pod_key, pod_skew, np.zeros(P, np.uint64), np.zeros((0, N), np.int32),
+                              np.zeros(N, np.uint64), np.zeros(0, np.int32), [])
+    all_nodes = nodes + other
+    spec_of, domains = _spread_domains(pods, constraints, all_nodes)
+    dom_bytes = {spec: dom.tobytes() for spec, dom in domains.items()}  # once per distinct domain requirement
+    key_id, keys, key_domain = {}, [], []
+    for i, c in constraints:
+        dom = domains[spec_of[i]]
+        key = (pods[i].namespace, c.selector, dom_bytes[spec_of[i]], c.min_domains)
+        k = key_id.get(key)
+        if k is None:
+            if len(keys) == MAX_TS_KEYS:
+                raise ValueError("more than %d distinct topology spread keys are not supported" % MAX_TS_KEYS)
+            k = key_id[key] = len(keys)
+            keys.append(key)
+            key_domain.append(dom)
+        pod_key[i] = k
+    K = len(keys)
+    # the selected pods: the pods to place and the running pods on the listed nodes, grouped by projection
+    row_ptr, run_idx = running_csr(all_nodes, running) if all_nodes and running else \
+        (np.zeros(len(all_nodes) + 1, np.int64), np.zeros(0, np.int32))
+    on_nodes = np.unique(run_idx)
+    everyone = pods + [running[j] for j in on_nodes.tolist()]
+    label_keys = sorted({key for _, sel, _, _ in keys if sel is not None for key, *_ in sel[0] + sel[1]})
+    group, proj, code_of = _pod_projection(everyone, label_keys)
+    column = {key: 1 + k for k, key in enumerate(label_keys)}
+    node_of_row = np.repeat(np.arange(len(all_nodes), dtype=np.int64), np.diff(row_ptr))
+    at = P + np.searchsorted(on_nodes, run_idx)  # a running pod is in `everyone` at P + its rank in on_nodes
+    pod_matches = np.zeros(P, dtype=np.uint64)
+    counts = np.zeros((K, len(all_nodes)), dtype=np.int64)
+    for k, (ns, sel, _, _) in enumerate(keys):
+        hit = _term_selects((frozenset((ns,)), sel), proj, code_of, column) if sel is not None else \
+            np.zeros(len(proj), bool)
+        pod_matches[hit[group[:P]]] |= np.uint64(1) << np.uint64(k)
+        rows = hit[group[at]] if len(run_idx) else np.zeros(0, bool)
+        counts[k] = np.bincount(node_of_row[rows], minlength=len(all_nodes))
+    for i, c in constraints:
+        k = int(pod_key[i])
+        pod_skew[i] = c.max_skew - int((int(pod_matches[i]) >> k) & 1)
+    node_domain = np.zeros(N, dtype=np.uint64)
+    floor = np.full(K, INT32_MAX, dtype=np.int32)
+    for k, dom in enumerate(key_domain):
+        node_domain[dom[:N]] |= np.uint64(1) << np.uint64(k)
+        outside = dom[N:]
+        if int(dom.sum()) < keys[k][3]:
+            floor[k] = 0
+        elif outside.any():
+            floor[k] = min(int(counts[k, N:][outside].min()), INT32_MAX)
+    node_count = np.minimum(counts[:, :N], INT32_MAX).astype(np.int32)
+    return TopologySpread(pod_key, pod_skew, pod_matches, node_count, node_domain, floor, keys)
+
+
+# ------------------------------------------------------------------------------------------------
 # K0: feasibility (capacity.is_possible over the pools)
 # ------------------------------------------------------------------------------------------------
 def feasible_pods(pods, agent_pools, classes=None):
@@ -726,12 +854,14 @@ def count_running_pods(nodes, running_pods):
 # ------------------------------------------------------------------------------------------------
 # first fit over nodes (Cluster.get_pending_pods)
 # ------------------------------------------------------------------------------------------------
-def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None, pod_affinity=None):
+def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None, pod_affinity=None, topology_spread=None):
     """returns placed[len(pods)] (node index or -1) and mutates node.used_capacity like count_pod.  With `classes`
     (selector_classes(pods, nodes, [])) a pod only takes a node that matches its nodeSelector.  With `anti_affinity`
     (anti_affinity(pods, nodes, running_pods)) a pod only takes a node its required anti-affinity does not block; the
     node masks are updated in place.  With `pod_affinity` (pod_affinity(pods, nodes, running_pods)) a pod only takes a
-    node its required pod affinity admits; node_has is updated in place."""
+    node its required pod affinity admits; node_has is updated in place.  With `topology_spread`
+    (topology_spread(pods, nodes, running_pods, other_nodes)) a pod only takes a node where its key's skew stays within
+    maxSkew; node_count is updated in place."""
     pods, nodes = list(pods), list(nodes)
     placed = np.full(len(pods), -1, dtype=np.int32)
     if not pods or not nodes:
@@ -746,7 +876,39 @@ def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None, pod_affinity=
     eng = get_engine()
     d_used = eng.dev(used, torch.float64)
     sel = classes is not None and not classes.trivial
-    if pod_affinity is not None and not pod_affinity.trivial:
+    if topology_spread is not None and not topology_spread.trivial:
+        ts = topology_spread
+        pa = pod_affinity if pod_affinity is not None and not pod_affinity.trivial else None
+        aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
+        d_nh = d_nc = d_nx = None
+        pa_args = aa_args = None
+        if pa is not None:
+            d_nh = eng.dev(pa.node_has.view(np.int64), torch.int64)
+            pa_args = tuple(eng.dev(a.view(np.int64), torch.int64) for a in (pa.pod_requires, pa.pod_self,
+                                                                               pa.pod_matches)) + (d_nh,)
+        if aa is not None:
+            d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
+            aa_args = (eng.dev(aa.pod_carries.view(np.int64), torch.int64),
+                       eng.dev(aa.pod_matches.view(np.int64), torch.int64), d_nc, d_nx)
+        d_cnt = eng.dev(np.ascontiguousarray(ts.node_count), torch.int32)
+        d_placed, _ = eng.first_fit_nodes_ts(eng.dev(req, torch.float64),
+                                             None if not bad.any() else eng.dev(ok_idx, torch.int32),
+                                             eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
+                                             len(ts.keys), eng.dev(ts.pod_key, torch.uint8),
+                                             eng.dev(ts.pod_skew, torch.int32),
+                                             eng.dev(ts.pod_matches.view(np.int64), torch.int64), d_cnt,
+                                             eng.dev(ts.node_domain.view(np.int64), torch.int64), ts.floor,
+                                             pa=pa_args, aa=aa_args,
+                                             **(dict(pod_class=eng.dev(classes.pod_class, torch.uint8),
+                                                     node_match=eng.dev(classes.node_match.view(np.int64), torch.int64),
+                                                     classes=classes.classes) if sel else {}))
+        ts.node_count[:] = d_cnt.cpu().numpy()
+        if pa is not None:
+            pa.node_has[:] = d_nh.cpu().numpy().view(np.uint64)
+        if aa is not None:
+            aa.node_carries[:] = d_nc.cpu().numpy().view(np.uint64)
+            aa.node_matches[:] = d_nx.cpu().numpy().view(np.uint64)
+    elif pod_affinity is not None and not pod_affinity.trivial:
         pa = pod_affinity
         aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
         d_nh = eng.dev(pa.node_has.view(np.int64), torch.int64)
@@ -825,13 +987,14 @@ def single_can_fit(node, resources):
 # fulfill_pending (bins)
 # ------------------------------------------------------------------------------------------------
 def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_provision, classes=None,
-            anti_affinity=None, pod_affinity=None, affinity_present=()):
+            anti_affinity=None, pod_affinity=None, affinity_present=(), topology_spread=None):
     """Scaler.fulfill_pending's packing + size arithmetic; pools already in visiting order.  With `classes`
     (selector_classes(unique_pods, [], ordered_pools)) a pool only takes the pods whose nodeSelector it matches.  With
     `anti_affinity` (anti_affinity(unique_pods)) a pod only takes a bin its required anti-affinity does not block.  With
     `pod_affinity` (pod_affinity(unique_pods)) a pod only takes a bin its required pod affinity admits;
     `affinity_present` holds the signatures the nodes already hold (PodAffinity.present_signatures of the node pass);
-    without it only the pods this call places count."""
+    without it only the pods this call places count.  With `topology_spread` (topology_spread(unique_pods)) a new node
+    takes at most maxSkew pods its key's selector selects, counting the pod itself."""
     from . import capacity
     units = [capacity.RESOURCE_SPEC[pool.instance_type] for pool in ordered_pools]
     dims = Dims([p.resources for p in unique_pods] + units)
@@ -844,7 +1007,22 @@ def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_pro
              np.asarray([min(pool.max_size, 2 ** 31 - 1) for pool in ordered_pools], dtype=np.int32),
              np.asarray([1 if pool.name in ignored_pool_names else 0 for pool in ordered_pools], dtype=np.uint8))
     sel = classes is not None and not classes.trivial
-    if pod_affinity is not None and not pod_affinity.trivial:
+    if topology_spread is not None and not topology_spread.trivial:
+        ts = topology_spread
+        pa = pod_affinity if pod_affinity is not None and not pod_affinity.trivial else None
+        aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
+        present = 0 if pa is None else sum(1 << k for k, sig in enumerate(pa.signatures) if sig in affinity_present)
+        res = eng.fulfill_pending_ts(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
+                                     len(ts.keys), eng.dev(ts.pod_key, torch.uint8), eng.dev(ts.pod_skew, torch.int32),
+                                     eng.dev(ts.pod_matches.view(np.int64), torch.int64),
+                                     pa=None if pa is None else tuple(eng.dev(a.view(np.int64), torch.int64) for a in (
+                                         pa.pod_requires, pa.pod_self, pa.pod_matches)),
+                                     present=present,
+                                     aa=None if aa is None else (eng.dev(aa.pod_carries.view(np.int64), torch.int64),
+                                                                 eng.dev(aa.pod_matches.view(np.int64), torch.int64)),
+                                     **(dict(pod_class=eng.dev(classes.pod_class, torch.uint8),
+                                             pool_match=classes.pool_match, classes=classes.classes) if sel else {}))
+    elif pod_affinity is not None and not pod_affinity.trivial:
         pa, aa = pod_affinity, anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
         present = sum(1 << k for k, sig in enumerate(pa.signatures) if sig in affinity_present)
         res = eng.fulfill_pending_pa(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
