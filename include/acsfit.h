@@ -523,6 +523,7 @@ ACSFIT_API acsfit_status acsfit_last_affinity_reruns(const acsfit_ctx *ctx, int6
  *   node_count    [dev] keys x N (key-major), read and written (node pass only; fulfill ignores it)
  *   node_domain   [dev] N (node pass only)
  *   floor         [host] keys (node pass only)
+ * acsfit_pending_admit_ts reads node_count (read only), node_domain, floor and keys, and none of the pod_* fields.
  * acsfit_first_fit_nodes_ts / acsfit_fulfill_pending_ts take the arguments of the *_pa forms with `sel`, `aa` and `pa`
  * all allowed to be NULL, plus `ts`.  They run the pod-affinity form of the pipeline kernel with the spread test
  * added, and refuse with ACSFIT_E_INVALID: a NULL `ts` or array that is read, keys outside [0, 64], a pod_key >= keys
@@ -556,6 +557,33 @@ ACSFIT_API acsfit_status acsfit_fulfill_pending_ts(acsfit_ctx *ctx, const double
                                                    int32_t *out_acc_pool, int32_t *out_bin_of,
                                                    int64_t *out_unaccounted, uint64_t *out_evals,
                                                    acsfit_stream_t stream);
+/*
+ * Pending-pod admission with hostname topology spread (opt-in), with or without anti-affinity and pod affinity:
+ * acsfit_pending_admit_pa's tests plus the spread test.  A signature (class, carries, matches, need, key, skew) admits
+ * node n when the enabled tests of acsfit_pending_admit_pa pass and key == 0xFF or node_count[key * N + n] <= skew +
+ * min(key), the rule of acsfit_topology_spread with nothing placed (each pending pod is judged on its own, so no
+ * minimum rises).  key and skew are the pod's pod_key and pod_skew.
+ *   run_carries, run_matches, sig_carries, sig_matches: all four NULL (no anti-affinity test) or given as in
+ *               acsfit_pending_admit
+ *   run_has, sig_need: both NULL (no affinity test) or given as in acsfit_pending_admit_pa
+ *   sig_key     [host] U bytes: the signature's key, 0xFF none; sig_skew [host] U int32 >= 0
+ *   ts          node_count (read only here), node_domain, floor and keys of acsfit_topology_spread over these N nodes;
+ *               pod_key, pod_skew and pod_matches are not read (the signatures carry key and skew).  node_count
+ *               must be 4-byte and node_domain 8-byte aligned
+ * The limit skew + min(key) is computed in 64 bits and clamped to INT32_MAX, so a key without any domain (min
+ * INT32_MAX) admits every node.  The other arguments are those of acsfit_pending_admit.  ACSFIT_E_INVALID: the
+ * refusals of acsfit_pending_admit_pa for the tests that run, a NULL ts, keys outside [0, 64], a NULL node_count or
+ * node_domain when N > 0 and keys > 0, a NULL floor when keys > 0, a NULL sig_key or sig_skew when U > 0, a sig_key
+ * >= keys other than 0xFF, a negative sig_skew, floor or node count, a misaligned node_count or node_domain; the flags
+ * are then left untouched.  acsfit_last_scan_launch reports the launch as kernel 5.
+ */
+ACSFIT_API acsfit_status acsfit_pending_admit_ts(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
+                                                 const uint64_t *run_matches, const uint64_t *run_has, int64_t N,
+                                                 const uint64_t *node_match, const uint8_t *sig_class,
+                                                 const uint64_t *sig_carries, const uint64_t *sig_matches,
+                                                 const uint64_t *sig_need, const uint8_t *sig_key,
+                                                 const int32_t *sig_skew, int U, const acsfit_topology_spread *ts,
+                                                 uint8_t *node_flags_inout, acsfit_stream_t stream);
 /* test hook: the rises the last *_ts call fixed, in order: out_pairs[2k] = key, out_pairs[2k + 1] = position (the
  * node pass's list entry after which the key's minimum rose; 2 * *out_rises entries; may be NULL) */
 ACSFIT_API acsfit_status acsfit_last_spread_rises(const acsfit_ctx *ctx, int64_t *out_rises, int64_t *out_pairs);
@@ -631,7 +659,8 @@ ACSFIT_API acsfit_status acsfit_last_launches(const acsfit_ctx *ctx, int *out, i
  *    grid (CTAs), S (idle thresholds; 0 for occupancy)}
  * acsfit_pending_admit reports {3, 0, 0, shared-memory bytes per CTA, warps per CTA, signatures per tile, grid, U};
  * acsfit_pending_admit_pa {4, 1 with the anti-affinity test (0 without), 0, shared-memory bytes per CTA, warps per CTA,
- * signatures per tile, grid, U}. */
+ * signatures per tile, grid, U}; acsfit_pending_admit_ts {5, 1 with the anti-affinity test | 2 with the affinity test,
+ * 0, shared-memory bytes per CTA, warps per CTA, signatures per tile, grid, U}. */
 #define ACSFIT_SCAN_FIELDS 8
 ACSFIT_API acsfit_status acsfit_last_scan_launch(const acsfit_ctx *ctx, int *out);
 

@@ -83,6 +83,8 @@ SIGNATURES = {
                                           c_vp, c_vp, c_vp, ctypes.c_uint64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                           c_vp, c_vp]),
     "acsfit_last_spread_rises": (c_int, [c_vp, c_vp, c_vp]),
+    "acsfit_pending_admit_ts": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                        c_vp, c_int, c_vp, c_vp, c_vp]),
 }
 
 

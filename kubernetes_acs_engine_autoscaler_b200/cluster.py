@@ -56,7 +56,8 @@ class Cluster(object):
                  acs_deployment='azuredeploy', scale_up=True, maintainance=True,
                  over_provision=5, dry_run=False, node_selectors=None, selector_node_states=None,
                  node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None,
-                 pod_affinity=None, pod_affinity_node_states=None, topology_spread=None):
+                 pod_affinity=None, pod_affinity_node_states=None, topology_spread=None,
+                 topology_spread_node_states=None):
         self.kubeconfig = kubeconfig
         # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
         # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
@@ -121,6 +122,14 @@ class Cluster(object):
         if topology_spread is None:
             topology_spread = os.environ.get('ACSFIT_TOPOLOGY_SPREAD', '0') not in ('', '0')
         self.topology_spread = bool(topology_spread)
+        # with topology spread on, also in maintain: a node is pod-pending only when some pod to schedule could land on it
+        # given its spread constraint, so a replica that may not stack beside its siblings does not freeze their nodes
+        # (opt-in; None: $ACSFIT_TOPOLOGY_SPREAD_NODE_STATES).  Combines with the other node-states switches.
+        if topology_spread_node_states is None:
+            topology_spread_node_states = os.environ.get('ACSFIT_TOPOLOGY_SPREAD_NODE_STATES', '0') not in ('', '0')
+        elif topology_spread_node_states and not self.topology_spread:
+            raise ValueError("topology_spread_node_states=True needs topology_spread on")
+        self.topology_spread_node_states = bool(topology_spread_node_states) and self.topology_spread
         self.other_nodes = []  # the listed nodes that are not agents (the master): domains of the spread constraints
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
@@ -228,7 +237,8 @@ class Cluster(object):
             selector_node_states=self.selector_node_states, node_taints=self.node_taints,
             pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity,
             anti_affinity_node_states=self.anti_affinity_node_states, pod_affinity=self.pod_affinity,
-            pod_affinity_node_states=self.pod_affinity_node_states, topology_spread=self.topology_spread)
+            pod_affinity_node_states=self.pod_affinity_node_states, topology_spread=self.topology_spread,
+            topology_spread_node_states=self.topology_spread_node_states, other_nodes=self.other_nodes)
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [

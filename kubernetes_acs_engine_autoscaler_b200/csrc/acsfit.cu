@@ -2694,22 +2694,46 @@ extern "C" acsfit_status acsfit_node_states(acsfit_ctx *ctx, const int64_t *row_
 
 static bool aligned8(const void *p) { return ((uintptr_t)p & 7u) == 0; }
 
-// acsfit_pending_admit and acsfit_pending_admit_pa: one validation, arena and launch.  `pa` is the entry point (its
-// launch record is kernel 4; acsfit_pending_admit's stays kernel 3).  The anti-affinity test runs when any of the four
+// acsfit_pending_admit, acsfit_pending_admit_pa and acsfit_pending_admit_ts: one validation, arena and launch.
+// `entry` is the entry point's launch record kernel (3, 4 or 5).  The anti-affinity test runs when any of the four
 // anti-affinity arrays is given (always, for acsfit_pending_admit); the run pair must then be given when there are rows
-// and the signature pair when U > 0.  The affinity test runs with `pa`.
-static acsfit_status pending_admit_impl(acsfit_ctx *ctx, bool pa, const int64_t *row_ptr,
+// and the signature pair when U > 0.  The affinity test runs for acsfit_pending_admit_pa, and for
+// acsfit_pending_admit_ts when run_has or sig_need is given.  The spread test runs for acsfit_pending_admit_ts: each
+// key's minimum over the listed domains comes from ts_domains_kernel, the host folds floor in and stages each
+// signature's limit, min(INT32_MAX, skew + min).
+static acsfit_status pending_admit_impl(acsfit_ctx *ctx, int entry, const int64_t *row_ptr,
                                         const uint64_t *run_carries, const uint64_t *run_matches,
                                         const uint64_t *run_has, int64_t N, const uint64_t *node_match,
                                         const uint8_t *sig_class, const uint64_t *sig_carries,
-                                        const uint64_t *sig_matches, const uint64_t *sig_need, int U,
+                                        const uint64_t *sig_matches, const uint64_t *sig_need, const uint8_t *sig_key,
+                                        const int32_t *sig_skew, int U, const acsfit_topology_spread *ts,
                                         uint8_t *node_flags_inout, cudaStream_t st)
 {
-    const char *what = pa ? "pending_admit_pa" : "pending_admit";
-    const bool aa = !pa || run_carries || run_matches || sig_carries || sig_matches;
+    const char *what = entry == 3 ? "pending_admit" : entry == 4 ? "pending_admit_pa" : "pending_admit_ts";
+    const bool aa = entry == 3 || run_carries || run_matches || sig_carries || sig_matches;
+    const bool pa = entry == 4 || (entry == 5 && (run_has || sig_need));
+    const bool tsf = entry == 5;
     if (N < 0 || U < 0 || (N > 0 && (!row_ptr || !node_flags_inout)) ||
         (N > 0 && U > 0 && (!sig_class || (aa && (!sig_carries || !sig_matches)) || (pa && !sig_need))))
         return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
+    const int keys = tsf && ts ? ts->keys : 0;
+    if (tsf) {
+        if (!ts) return fail(ctx, ACSFIT_E_INVALID, "%s: topology-spread arrays missing", what);
+        if (keys < 0 || keys > ACSFIT_MAX_TS_KEYS)
+            return fail(ctx, ACSFIT_E_INVALID, "%s: %d spread keys, at most %d", what, keys, ACSFIT_MAX_TS_KEYS);
+        if ((N > 0 && keys > 0 && (!ts->node_count || !ts->node_domain)) || (keys > 0 && !ts->floor) ||
+            (U > 0 && (!sig_key || !sig_skew)))
+            return fail(ctx, ACSFIT_E_INVALID, "%s: topology-spread field missing", what);
+        for (int k = 0; k < keys; ++k)
+            if (ts->floor[k] < 0)
+                return fail(ctx, ACSFIT_E_INVALID, "%s: floor[%d] = %d is negative", what, k, ts->floor[k]);
+        for (int u = 0; u < U; ++u)
+            if ((sig_key[u] != kAdmitNoKey && sig_key[u] >= keys) || sig_skew[u] < 0)
+                return fail(ctx, ACSFIT_E_INVALID, "%s: signature %d has key %d and skew %d (%d keys)", what, u,
+                            sig_key[u], sig_skew[u], keys);
+        if (((uintptr_t)ts->node_count & 3u) != 0 || ((uintptr_t)ts->node_domain & 7u) != 0)
+            return fail(ctx, ACSFIT_E_INVALID, "%s: node_count must be 4-byte and node_domain 8-byte aligned", what);
+    }
     if (N == 0) return ACSFIT_OK;
     if ((N + kAdmitBlock - 1) / kAdmitBlock > INT32_MAX)
         return fail(ctx, ACSFIT_E_INVALID, "%s: N=%lld nodes is too many", what, (long long)N);
@@ -2731,7 +2755,8 @@ static acsfit_status pending_admit_impl(acsfit_ctx *ctx, bool pa, const int64_t 
         return fail(ctx, ACSFIT_E_INVALID, "%s: %lld rows but a NULL run mask array", what,
                     (long long)(ends[1] - ends[0]));
     const size_t Uq = (size_t)std::max(U, 1);
-    TRY(arena_reserve(ctx, Uq * ((aa ? 2 : 0) * sizeof(uint64_t) + (pa ? sizeof(uint64_t) : 0) + 1) + 1024, st));
+    TRY(arena_reserve(ctx, Uq * ((aa ? 2 : 0) * sizeof(uint64_t) + (pa ? sizeof(uint64_t) : 0) + 1) + 1024 +
+                               (tsf ? Uq * (1 + sizeof(int32_t)) + sizeof(int) * (2 * 64 + 1) + 1024 : 0), st));
     ctx->arena_off = 0;
     unsigned long long *d_carries = nullptr, *d_matches = nullptr, *d_need = nullptr;
     if (aa) {
@@ -2745,23 +2770,67 @@ static acsfit_status pending_admit_impl(acsfit_ctx *ctx, bool pa, const int64_t 
         d_need = need;
     }
     TAKE(d_class, uint8_t, Uq);
+    uint8_t *d_key = nullptr;
+    int32_t *d_limit = nullptr;
+    if (tsf) {
+        TAKE(key, uint8_t, Uq);
+        TAKE(limit, int32_t, Uq);
+        d_key = key;
+        d_limit = limit;
+    }
+    if (tsf && keys > 0) {  // refuse negative counts, then each key's minimum over the listed domains
+        TAKE(scratch, int, 2 * 64 + 1);
+        int init[2 * 64 + 1];
+        for (int k = 0; k < 64; ++k) {
+            init[k] = INT_MAX;
+            init[64 + k] = 0;
+        }
+        init[128] = 0;
+        CUDA_TRY(cudaMemcpyAsync(scratch, init, sizeof init, cudaMemcpyHostToDevice, st));
+        ts_check_kernel<<<grid_for(ctx, N * keys, 256), 256, 0, st>>>(nullptr, nullptr, nullptr, 0, keys,
+                                                                      ts->node_count, N * keys, scratch + 128);
+        ts_domains_kernel<<<grid_for(ctx, N * keys, 256), 256, 0, st>>>(
+            ts->node_count, reinterpret_cast<const unsigned long long *>(ts->node_domain), N, keys, nullptr, scratch,
+            scratch + 64, nullptr);
+        ctx->launches += 2;
+        int got[2 * 64 + 1];
+        CUDA_TRY(cudaMemcpyAsync(got, scratch, sizeof got, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        CUDA_TRY(cudaGetLastError());
+        if (got[128] & 16) return fail(ctx, ACSFIT_E_INVALID, "%s: a node count is negative", what);
+        std::vector<int32_t> limit(U);
+        for (int u = 0; u < U; ++u) {
+            const int k = sig_key[u];
+            const long long m = k == kAdmitNoKey ? 0 : std::min(ts->floor[k], got[k]);
+            limit[u] = (int32_t)std::min<long long>(INT32_MAX, (long long)sig_skew[u] + m);
+        }
+        if (U > 0) CUDA_TRY(cudaMemcpyAsync(d_limit, limit.data(), sizeof(int32_t) * U, cudaMemcpyHostToDevice, st));
+    } else if (tsf && U > 0) {  // no key: every signature is 0xFF and its limit is never read
+        CUDA_TRY(cudaMemsetAsync(d_limit, 0, sizeof(int32_t) * U, st));
+    }
     if (U > 0) {
         if (aa) {
             CUDA_TRY(cudaMemcpyAsync(d_carries, sig_carries, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
             CUDA_TRY(cudaMemcpyAsync(d_matches, sig_matches, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
         }
         if (pa) CUDA_TRY(cudaMemcpyAsync(d_need, sig_need, sizeof(uint64_t) * U, cudaMemcpyHostToDevice, st));
+        if (tsf) CUDA_TRY(cudaMemcpyAsync(d_key, sig_key, U, cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(d_class, sig_class, U, cudaMemcpyHostToDevice, st));
     }
     const int grid = (int)((N + kAdmitBlock - 1) / kAdmitBlock);
-    auto kernel = !pa ? pending_admit_kernel<true, false>
-                      : aa ? pending_admit_kernel<true, true> : pending_admit_kernel<false, true>;
+    auto kernel = !tsf ? (!pa ? pending_admit_kernel<true, false, false>
+                              : aa ? pending_admit_kernel<true, true, false> : pending_admit_kernel<false, true, false>)
+                       : aa ? (pa ? pending_admit_kernel<true, true, true> : pending_admit_kernel<true, false, true>)
+                            : (pa ? pending_admit_kernel<false, true, true> : pending_admit_kernel<false, false, true>);
     kernel<<<grid, kAdmitBlock, 0, st>>>(
         row_ptr, reinterpret_cast<const unsigned long long *>(run_carries),
         reinterpret_cast<const unsigned long long *>(run_matches), N,
         reinterpret_cast<const unsigned long long *>(node_match), d_class, d_carries, d_matches, U, node_flags_inout,
-        reinterpret_cast<const unsigned long long *>(run_has), d_need);
-    if (pa)
+        reinterpret_cast<const unsigned long long *>(run_has), d_need, d_key, d_limit, keys > 0 ? ts->node_count : nullptr);
+    if (tsf)
+        ctx->scan_rec = {5, (aa ? 1 : 0) | (pa ? 2 : 0), 0, admit_smem_ts(aa, pa), kAdmitBlock / 32, kAdmitBlock, grid,
+                         U};
+    else if (pa)
         ctx->scan_rec = {4, aa ? 1 : 0, 0, aa ? kAdmitSmemAaPa : kAdmitSmemPa, kAdmitBlock / 32, kAdmitBlock, grid, U};
     else
         ctx->scan_rec = {3, kScanPerThread, 0, kAdmitSmem, kAdmitBlock / 32, kAdmitBlock, grid, U};
@@ -2778,8 +2847,9 @@ extern "C" acsfit_status acsfit_pending_admit(acsfit_ctx *ctx, const int64_t *ro
                                               acsfit_stream_t stream)
 {
     TRY(enter(ctx, 1));
-    return pending_admit_impl(ctx, false, row_ptr, run_carries, run_matches, nullptr, N, node_match, sig_class,
-                              sig_carries, sig_matches, nullptr, U, node_flags_inout, (cudaStream_t)stream);
+    return pending_admit_impl(ctx, 3, row_ptr, run_carries, run_matches, nullptr, N, node_match, sig_class,
+                              sig_carries, sig_matches, nullptr, nullptr, nullptr, U, nullptr, node_flags_inout,
+                              (cudaStream_t)stream);
 }
 
 extern "C" acsfit_status acsfit_pending_admit_pa(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
@@ -2790,8 +2860,23 @@ extern "C" acsfit_status acsfit_pending_admit_pa(acsfit_ctx *ctx, const int64_t 
                                                  acsfit_stream_t stream)
 {
     TRY(enter(ctx, 1));
-    return pending_admit_impl(ctx, true, row_ptr, run_carries, run_matches, run_has, N, node_match, sig_class,
-                              sig_carries, sig_matches, sig_need, U, node_flags_inout, (cudaStream_t)stream);
+    return pending_admit_impl(ctx, 4, row_ptr, run_carries, run_matches, run_has, N, node_match, sig_class,
+                              sig_carries, sig_matches, sig_need, nullptr, nullptr, U, nullptr, node_flags_inout,
+                              (cudaStream_t)stream);
+}
+
+extern "C" acsfit_status acsfit_pending_admit_ts(acsfit_ctx *ctx, const int64_t *row_ptr, const uint64_t *run_carries,
+                                                 const uint64_t *run_matches, const uint64_t *run_has, int64_t N,
+                                                 const uint64_t *node_match, const uint8_t *sig_class,
+                                                 const uint64_t *sig_carries, const uint64_t *sig_matches,
+                                                 const uint64_t *sig_need, const uint8_t *sig_key,
+                                                 const int32_t *sig_skew, int U, const acsfit_topology_spread *ts,
+                                                 uint8_t *node_flags_inout, acsfit_stream_t stream)
+{
+    TRY(enter(ctx, 1));
+    return pending_admit_impl(ctx, 5, row_ptr, run_carries, run_matches, run_has, N, node_match, sig_class,
+                              sig_carries, sig_matches, sig_need, sig_key, sig_skew, U, ts, node_flags_inout,
+                              (cudaStream_t)stream);
 }
 
 static acsfit_status maintain_actions_impl(acsfit_ctx *ctx, uint8_t *io_state, const int32_t *node_pool, int64_t N,

@@ -29,7 +29,9 @@ struct ScanPlan {
 // one acsfit_last_scan_launch record (ACSFIT_SCAN_FIELDS ints, in this order), written where the kernel is launched
 struct ScanLaunch {
     int kernel;  // 0 none, 1 occupancy (K1), 2 node states (K6), 3 pending admission (acsfit_pending_admit),
-                 // 4 pending admission with pod affinity (acsfit_pending_admit_pa)
+                 // 4 pending admission with pod affinity (acsfit_pending_admit_pa),
+                 // 5 pending admission with topology spread (acsfit_pending_admit_ts; form: 1 anti-affinity | 2 pod
+                 // affinity)
     int form, D, bytes_per_warp, warps, chunk;
     int grid;    // CTAs launched
     int S;       // idle thresholds (0 for K1)

@@ -298,6 +298,32 @@ class Engine(object):
                                                       _ptr(node_flags), self._stream()))
         return node_flags
 
+    def pending_admit_ts(self, row_ptr, run_carries, run_matches, run_has, node_match, sig_class, sig_carries,
+                         sig_matches, sig_need, sig_key, sig_skew, keys, node_count, node_domain, floor, node_flags):
+        """pending_admit_pa with the topology-spread test (include/acsfit.h, acsfit_pending_admit_ts): a signature with
+        a key (sig_key != 0xFF) admits a node only when the node's count of that key is at most sig_skew plus the key's
+        minimum.  sig_key uint8 and sig_skew int32 host arrays of length U; node_count int32 [keys, N] and node_domain
+        uint64 [N] (stored as int64) on the device, floor int32 [keys] host.  The anti-affinity quadruple and the
+        pod-affinity pair (run_has, sig_need) are each all None (that test does not run) or all given."""
+        N = node_flags.shape[0]
+        sig_class, sig_key, sig_skew = _np(sig_class, np.uint8), _np(sig_key, np.uint8), _np(sig_skew, np.int32)
+        U = sig_class.shape[0]
+        assert sig_key.shape == sig_skew.shape == (U,)
+        if sig_carries is not None or sig_matches is not None:
+            sig_carries, sig_matches = _np(sig_carries, np.uint64), _np(sig_matches, np.uint64)
+            assert sig_carries.shape == sig_matches.shape == (U,)
+        if sig_need is not None:
+            sig_need = _np(sig_need, np.uint64)
+            assert sig_need.shape == (U,)
+        ts, keep_t = self._spread(keys, None, None, None, node_count, node_domain, floor)
+        self._check(self._lib.acsfit_pending_admit_ts(self._ctx, _ptr(row_ptr), _ptr(run_carries), _ptr(run_matches),
+                                                      _ptr(run_has), N, _ptr(node_match), _ptr(sig_class),
+                                                      _ptr(sig_carries), _ptr(sig_matches), _ptr(sig_need),
+                                                      _ptr(sig_key), _ptr(sig_skew), U,
+                                                      ctypes.cast(ctypes.byref(ts), ctypes.c_void_p), _ptr(node_flags),
+                                                      self._stream()))
+        return node_flags
+
     def maintain_actions(self, state, node_pool, budget0, pool_scalable, dry_run):
         """engine_scaler.py:133-182 decisions. `state` uint8[N] device is rewritten; returns action uint8[N]."""
         N = state.shape[0]

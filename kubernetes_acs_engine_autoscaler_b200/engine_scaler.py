@@ -24,7 +24,7 @@ class EngineScaler(Scaler):
                  deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
                  selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False,
                  anti_affinity_node_states=False, pod_affinity=False, pod_affinity_node_states=False,
-                 topology_spread=False):
+                 topology_spread=False, topology_spread_node_states=False, other_nodes=()):
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
         self.node_selectors = node_selectors
@@ -36,6 +36,8 @@ class EngineScaler(Scaler):
         self.pod_affinity = pod_affinity
         self.pod_affinity_node_states = pod_affinity_node_states
         self.topology_spread = topology_spread
+        self.topology_spread_node_states = topology_spread_node_states
+        self.other_nodes = list(other_nodes)
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template
         for pool_name in ignore_pools.split(','):  # '' -> {'': True}, like the reference (:31-32)

@@ -82,6 +82,11 @@ class Scaler(object):
         self.pod_affinity_node_states = False
         # hostname topology spread (DoNotSchedule) in the bins of fulfill_pending (Cluster(topology_spread=...))
         self.topology_spread = False
+        # with topology spread: POD_PENDING only when some pod to schedule could land on the node given its spread
+        # constraint (Cluster(topology_spread_node_states=...))
+        self.topology_spread_node_states = False
+        # the listed nodes that are not agents (the master): domains of the spread constraints
+        self.other_nodes = []
 
     def get_agent_pools(self, nodes):
         raise NotImplementedError()
@@ -97,30 +102,40 @@ class Scaler(object):
         return ~snapshot.pending_match(pods_to_schedule, nodes, taints=self.node_taints, affinity=self.node_affinity)
 
     def pending_flags(self, nodes, pods_lists, pods_to_schedule, running_pods, agent_pools=None):
-        """the keywords `no_match` and `admit` of snapshot.node_states.  With anti_affinity_node_states or
-        pod_affinity_node_states on, something to schedule and some term that can exclude a pod to schedule, the GPU
-        decides which nodes some pod to schedule is admitted to (snapshot.pending_admit: the enabled tests, node
-        selectors included when selector_node_states is on); otherwise no_pending_match decides.  A self-affine group
-        may bootstrap while no pod of `running_pods` on a node of `agent_pools` matches it (None: no pod of
-        `pods_lists`)."""
+        """the keywords `no_match` and `admit` of snapshot.node_states.  With anti_affinity_node_states,
+        pod_affinity_node_states or topology_spread_node_states on, something to schedule and some term or constraint
+        that can exclude a pod to schedule, the GPU decides which nodes some pod to schedule is admitted to
+        (snapshot.pending_admit: the enabled tests, node selectors included when selector_node_states is on);
+        otherwise no_pending_match decides.  A self-affine group may bootstrap while no pod of `running_pods` on a node
+        of `agent_pools` matches it (None: no pod of `pods_lists`).  The spread minimums count the nodes of
+        `agent_pools` outside `nodes` and self.other_nodes as domains (None: `nodes` alone)."""
         admit = None
-        if (self.anti_affinity_node_states or self.pod_affinity_node_states) and pods_to_schedule:
+        if (self.anti_affinity_node_states or self.pod_affinity_node_states or self.topology_spread_node_states) and \
+                pods_to_schedule:
             agent_nodes = None
             if self.pod_affinity_node_states and agent_pools is not None:
                 agent_nodes = [n for pool in agent_pools for n in pool.nodes]
+            other_nodes = ()
+            if self.topology_spread_node_states and agent_pools is not None:
+                listed = {n.name for n in nodes}
+                other_nodes = [n for pool in agent_pools for n in pool.nodes if n.name not in listed] + \
+                    list(self.other_nodes)
             admit = snapshot.pending_admit(pods_to_schedule, running_pods, nodes, pods_lists,
                                            selectors=self.selector_node_states, taints=self.node_taints,
                                            affinity=self.node_affinity, anti_affinity=self.anti_affinity_node_states,
-                                           pod_affinity=self.pod_affinity_node_states, agent_nodes=agent_nodes)
+                                           pod_affinity=self.pod_affinity_node_states, agent_nodes=agent_nodes,
+                                           topology_spread=self.topology_spread_node_states, other_nodes=other_nodes)
         if admit is not None:
             return {"no_match": None, "admit": admit}
         return {"no_match": self.no_pending_match(nodes, pods_to_schedule), "admit": None}
 
     def get_node_state(self, node, node_pods, pods_to_schedule):
         """ClusterNodeState of one node (scaler.py:61-114): a one-node launch of the idle scan.
-        EngineScaler.maintain classifies all nodes in a single launch instead.  The anti-affinity and pod-affinity
-        rules see only `node_pods`: with pod_affinity_node_states on, a self-affine group may bootstrap here unless one
-        of `node_pods` matches it, whereas maintain looks for a match on every agent node."""
+        EngineScaler.maintain classifies all nodes in a single launch instead.  The anti-affinity, pod-affinity and
+        topology-spread rules see only `node` and `node_pods`: with pod_affinity_node_states on, a self-affine group may
+        bootstrap here unless one of `node_pods` matches it, whereas maintain looks for a match on every agent node;
+        with topology_spread_node_states on, a key's minimum is the node's own count (0 when the key has fewer domains
+        than its minDomains), whereas maintain takes it over every listed node."""
         node_pods = list(node_pods)
         code = snapshot.node_states([node], [node_pods], bool(pods_to_schedule), self.idle_threshold,
                                     **self.pending_flags([node], [node_pods], pods_to_schedule, node_pods))

@@ -782,6 +782,9 @@ def topology_spread(pods, nodes=(), running_pods=(), other_nodes=()):
     return TopologySpread(pod_key, pod_skew, pod_matches, node_count, node_domain, floor, keys)
 
 
+_topology_spread = topology_spread  # (pending_admit's keyword of the same name hides it there)
+
+
 # ------------------------------------------------------------------------------------------------
 # K0: feasibility (capacity.is_possible over the pools)
 # ------------------------------------------------------------------------------------------------
@@ -1101,14 +1104,15 @@ def node_age_seconds(node, now_by_tz=None):
 
 
 class PendingAdmit(object):
-    """what acsfit_pending_admit(_pa) reads beside node_states' table: row_carries / row_matches uint64[R] (one per row
-    of the table; None without the anti-affinity test), row_has uint64[R] (None without the pod-affinity test),
+    """what acsfit_pending_admit(_pa, _ts) reads beside node_states' table: row_carries / row_matches uint64[R] (one
+    per row of the table; None without the anti-affinity test), row_has uint64[R] (None without the pod-affinity test),
     node_match uint64[N] class masks or None (every pod matches every node), and the U distinct signatures (class,
-    carries, matches, need) of the pods to schedule: sig_class uint8[U], sig_carries / sig_matches / sig_need uint64[U]
-    (None without the test they belong to)."""
+    carries, matches, need, key, skew) of the pods to schedule: sig_class uint8[U], sig_carries / sig_matches /
+    sig_need uint64[U], sig_key uint8[U] and sig_skew int32[U] (None without the test they belong to).  With the
+    spread test, node_count int32[keys, N], node_domain uint64[N] and floor int32[keys] are topology_spread's."""
 
     def __init__(self, row_carries, row_matches, node_match, sig_class, sig_carries, sig_matches, row_has=None,
-                 sig_need=None):
+                 sig_need=None, sig_key=None, sig_skew=None, node_count=None, node_domain=None, floor=None):
         self.row_carries = row_carries
         self.row_matches = row_matches
         self.node_match = node_match
@@ -1117,10 +1121,15 @@ class PendingAdmit(object):
         self.sig_matches = sig_matches
         self.row_has = row_has
         self.sig_need = sig_need
+        self.sig_key = sig_key
+        self.sig_skew = sig_skew
+        self.node_count = node_count
+        self.node_domain = node_domain
+        self.floor = floor
 
 
 def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints=False, affinity=False,
-                  anti_affinity=True, pod_affinity=False, agent_nodes=None):
+                  anti_affinity=True, pod_affinity=False, agent_nodes=None, topology_spread=False, other_nodes=()):
     """the PendingAdmit of node_states(admit=...): node n stays pod-pending only when some pod of `pods` (the pods to
     schedule) passes every enabled test against pods_lists[n] (the node's pods, objects of `running_pods`):
     * `anti_affinity`: no pod of the node blocks it and it blocks none of them (anti_affinity_rows' masks);
@@ -1128,10 +1137,14 @@ def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints
       bootstrap a self-affine group: it matches its own signature and no pod of `running_pods` on `agent_nodes` does
       (pod_affinity_rows' masks; `agent_nodes` None: the pods of the table).  The bootstrap is folded into the need:
       need = 0 when requires & present == 0 and self != 0, need = requires otherwise;
+    * `topology_spread`: it has no honoured spread constraint, or the node's count of its key is at most its skew plus
+      the key's minimum (topology_spread(pods, nodes, running_pods, other_nodes)'s keys, skews, counts, domains and
+      floor; each pod is judged on its own, nothing is placed);
     * `selectors`: it matches the node as pending_match(pods, nodes, taints, affinity) decides (the classes are
       selector_classes(pods, nodes, [], taints, affinity)'s; ValueError above 64).
-    None when no enabled test can exclude a pod to schedule (no anti-affinity term is kept and no need is nonzero):
-    pending_match alone decides.  Without a nonzero need the table is the anti-affinity one (acsfit_pending_admit)."""
+    None when no enabled test can exclude a pod to schedule (no anti-affinity term is kept, no need is nonzero and no
+    pod has a spread key): pending_match alone decides.  Without a nonzero need and a key the table is the
+    anti-affinity one (acsfit_pending_admit); without a key it is the one of acsfit_pending_admit_pa."""
     pods = list(pods)
     row_carries = row_matches = row_has = None
     columns = []
@@ -1146,6 +1159,13 @@ def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints
         if need.any():
             row_has = rh
             columns.append(need)
+    ts = None
+    if topology_spread:
+        ts = _topology_spread(pods, nodes, running_pods, other_nodes)
+        if ts.trivial:
+            ts = None
+        else:
+            columns += [ts.pod_key.astype(np.uint64), ts.pod_skew.astype(np.uint64)]
     if not columns:
         return None
     pod_class, node_match = np.zeros(len(pods), dtype=np.uint8), None
@@ -1155,17 +1175,22 @@ def pending_admit(pods, running_pods, nodes, pods_lists, selectors=False, taints
             pod_class, node_match = classes.pod_class, classes.node_match
     sig = np.unique(np.stack([pod_class.astype(np.uint64)] + columns, axis=1), axis=0)
     col = lambda k: np.ascontiguousarray(sig[:, k])  # noqa: E731
-    aa = row_carries is not None
-    return PendingAdmit(row_carries, row_matches, node_match, sig[:, 0].astype(np.uint8), col(1) if aa else None,
-                        col(2) if aa else None, row_has, col(len(columns)) if row_has is not None else None)
+    aa, pa = row_carries is not None, row_has is not None
+    adm = PendingAdmit(row_carries, row_matches, node_match, sig[:, 0].astype(np.uint8), col(1) if aa else None,
+                       col(2) if aa else None, row_has, col(1 + 2 * aa) if pa else None)
+    if ts is not None:
+        k = 1 + 2 * aa + pa
+        adm.sig_key, adm.sig_skew = col(k).astype(np.uint8), col(k + 1).astype(np.int32)
+        adm.node_count, adm.node_domain, adm.floor = ts.node_count, ts.node_domain, ts.floor
+    return adm
 
 
 def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None, admit=None):
     """state code per node (include/acsfit.h ACSFIT_ST_*); pods_lists[n] = the node's pods in order.  `no_match`
     (bool[N], optional): nodes no pod to schedule matches (~pending_match); they are classified as if there were no
     pod to schedule (ACSFIT_NODEF_NO_PENDING_MATCH).  `admit` (pending_admit(..., pods_lists=pods_lists), optional):
-    the same flag for the nodes that no pod to schedule is admitted to, set on the GPU (acsfit_pending_admit, or
-    acsfit_pending_admit_pa when the table has row_has)."""
+    the same flag for the nodes that no pod to schedule is admitted to, set on the GPU (acsfit_pending_admit,
+    acsfit_pending_admit_pa when the table has row_has, acsfit_pending_admit_ts when it has sig_key)."""
     nodes = list(nodes)
     if not nodes:
         return np.zeros(0, dtype=np.uint8)
@@ -1188,10 +1213,16 @@ def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None, a
     d_row_ptr, d_node_flags = eng.dev(row_ptr, torch.int64), eng.dev(node_flags, torch.uint8)
     if admit is not None:
         rows = admit.row_carries if admit.row_carries is not None else admit.row_has
-        if len(rows) != len(flat):
+        if rows is not None and len(rows) != len(flat):
             raise ValueError("pending_admit masks of %d pods for a table of %d" % (len(rows), len(flat)))
         dev_masks = lambda a: None if a is None else eng.dev(a.view(np.int64), torch.int64)  # noqa: E731
-        if admit.row_has is None:
+        if admit.sig_key is not None:
+            eng.pending_admit_ts(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
+                                 dev_masks(admit.row_has), dev_masks(admit.node_match), admit.sig_class,
+                                 admit.sig_carries, admit.sig_matches, admit.sig_need, admit.sig_key, admit.sig_skew,
+                                 admit.node_count.shape[0], eng.dev(admit.node_count, torch.int32),
+                                 dev_masks(admit.node_domain), admit.floor, d_node_flags)
+        elif admit.row_has is None:
             eng.pending_admit(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
                               dev_masks(admit.node_match), admit.sig_class, admit.sig_carries, admit.sig_matches,
                               d_node_flags)

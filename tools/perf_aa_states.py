@@ -1,12 +1,16 @@
 #!/usr/bin/env python3
-"""developer probe: cost of node states with pod anti-affinity and pod affinity (Cluster(anti_affinity_node_states=True),
-Cluster(pod_affinity_node_states=True)).
+"""developer probe: cost of node states with pod anti-affinity, pod affinity and hostname topology spread
+(Cluster(anti_affinity_node_states=True), Cluster(pod_affinity_node_states=True),
+Cluster(topology_spread_node_states=True)).
 
   kernel   for each form of --forms (`aa`: acsfit_pending_admit; `pa`: acsfit_pending_admit_pa without the anti-affinity
-           masks; `aa+pa`: acsfit_pending_admit_pa with them) at --nodes nodes holding --rows running-pod rows, for each
-           U of --sigs, on two tables: `typical` (signature u carries, is selected by and needs term / signature u % 64;
-           half the running pods belong to one of 64 such deployments, so most nodes are admitted by one of the first
-           signatures) and `none` (no signature admits any node with pods: every thread walks the whole table).  Per
+           masks; `aa+pa`: acsfit_pending_admit_pa with them; `ts`: acsfit_pending_admit_ts with the spread test alone;
+           `aa+pa+ts`: acsfit_pending_admit_ts with all three tests) at --nodes nodes holding --rows running-pod rows,
+           for each U of --sigs, on two tables: `typical` (signature u carries, is selected by and needs term /
+           signature u % 64 and spreads over key u % 64 with maxSkew 1; half the running pods belong to one of 64 such
+           deployments, counted on their node under their key, so most nodes are admitted by one of the first
+           signatures) and `none` (no signature admits any node with pods: every thread walks the whole table; for
+           `ts`, every node counts one pod of every key and the floor is 0).  Per
            call: median CUDA-event time of the entry point (table upload, row_ptr read-back, kernel) over --reps calls
            after --warmup; per kernel: the device time torch.profiler records for pending_admit_kernel in a separate run.
   host     snapshot.pending_admit for U pods to schedule against the same number of running pods and nodes (CPU
@@ -60,6 +64,24 @@ def table(N, R, U, kind, seed=5):
     return row_ptr, rc, rm, rh, np.zeros(U, np.uint8), car, mat, need
 
 
+def spread(N, R, U, kind, row_ptr, seed=5):
+    """sig_key, sig_skew, node_count [64, N], node_domain, floor of the `ts` forms"""
+    rng = np.random.default_rng([seed, 1])
+    if kind == "typical":
+        key = rng.integers(0, 64, size=R)
+        grouped = rng.random(R) < 0.5
+        node_of = np.repeat(np.arange(N), np.diff(row_ptr))
+        count = np.zeros((64, N), np.int32)
+        np.add.at(count, (key[grouped], node_of[grouped]), 1)
+        floor = np.full(64, 2 ** 31 - 1, np.int32)
+        skew = np.ones(U, np.int32)
+    else:
+        count = np.ones((64, N), np.int32)
+        floor = np.zeros(64, np.int32)
+        skew = np.zeros(U, np.int32)
+    return (np.arange(U) % 64).astype(np.uint8), skew, count, np.full(N, ~np.uint64(0)), floor
+
+
 def kernel(args):
     import torch
     from kubernetes_acs_engine_autoscaler_b200.engine import Engine
@@ -71,12 +93,21 @@ def kernel(args):
             d_rp, d_rc, d_rm = eng.dev(row_ptr, i64), eng.dev(rc.view(np.int64), i64), eng.dev(rm.view(np.int64), i64)
             d_rh = eng.dev(rh.view(np.int64), i64)
             flags = eng.dev(np.zeros(args.nodes, np.uint8), torch.uint8)
+            if form.endswith("ts"):
+                key, skew, count, domain, floor = spread(args.nodes, args.rows, U, kind, row_ptr)
+                d_count, d_domain = eng.dev(count, torch.int32), eng.dev(domain.view(np.int64), i64)
 
             def call():
                 if form == "aa":
                     eng.pending_admit(d_rp, d_rc, d_rm, None, cls, car, mat, flags)
                 elif form == "pa":
                     eng.pending_admit_pa(d_rp, None, None, d_rh, None, cls, None, None, need, flags)
+                elif form == "ts":
+                    eng.pending_admit_ts(d_rp, None, None, None, None, cls, None, None, None, key, skew, 64, d_count,
+                                         d_domain, floor, flags)
+                elif form == "aa+pa+ts":
+                    eng.pending_admit_ts(d_rp, d_rc, d_rm, d_rh, None, cls, car, mat, need, key, skew, 64, d_count,
+                                         d_domain, floor, flags)
                 else:
                     eng.pending_admit_pa(d_rp, d_rc, d_rm, d_rh, None, cls, car, mat, need, flags)
             for _ in range(args.warmup):
@@ -95,7 +126,7 @@ def kernel(args):
                     call()
                 torch.cuda.synchronize()
             dev_us = [e.self_device_time_total / e.count for e in prof.key_averages() if "pending_admit_kernel" in e.key]
-            print("kernel %-5s %-7s N=%d rows=%d U=%-5d call %.3f ms (median of %d)  kernel %s  flagged %d" % (
+            print("kernel %-8s %-7s N=%d rows=%d U=%-5d call %.3f ms (median of %d)  kernel %s  flagged %d" % (
                 form, kind, args.nodes, args.rows, U, statistics.median(times), args.reps,
                 "%.3f ms" % (dev_us[0] / 1000.0) if dev_us else "n/a", flagged), flush=True)
 
@@ -136,7 +167,8 @@ def main():
     ap.add_argument("--nodes", type=int, default=1_000_000)
     ap.add_argument("--rows", type=int, default=10_000_000)
     ap.add_argument("--sigs", type=int, nargs="+", default=[1, 64, 4096])
-    ap.add_argument("--forms", nargs="+", choices=("aa", "pa", "aa+pa"), default=["aa", "pa", "aa+pa"])
+    ap.add_argument("--forms", nargs="+", choices=("aa", "pa", "aa+pa", "ts", "aa+pa+ts"),
+                    default=["aa", "pa", "aa+pa", "ts", "aa+pa+ts"])
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
