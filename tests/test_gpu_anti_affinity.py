@@ -46,11 +46,19 @@ def layout_case(name):
 
 @functools.lru_cache(maxsize=None)
 def oracle_of(key):
-    c = case(*key) if isinstance(key, tuple) else layout_case(key)
+    return oracle_of_case(case(*key) if isinstance(key, tuple) else layout_case(key))
+
+
+def oracle_of_case(c, pod_idx=None):
+    """the oracle over the req rows `pod_idx` in that order (None: every row); placements are in list positions, and
+    "pend" holds the req rows of the pods left pending, in list order"""
     used, nc, nx = c["used0"].copy(), c["node_carries0"].copy(), c["node_matches0"].copy()
-    placed, calls = aa_oracle.first_fit_nodes_aa(c["req"], c["cap_type"], c["node_type"], used, c["pod_carries"],
-                                                 c["pod_matches"], nc, nx, c.get("node_match"), c.get("pod_class"))
-    pend = np.nonzero(placed < 0)[0]
+    rows = np.arange(len(c["req"])) if pod_idx is None else np.asarray(pod_idx)
+    placed, calls = aa_oracle.first_fit_nodes_aa(c["req"][rows], c["cap_type"], c["node_type"], used,
+                                                 c["pod_carries"][rows], c["pod_matches"][rows], nc, nx,
+                                                 c.get("node_match"),
+                                                 None if "pod_class" not in c else c["pod_class"][rows])
+    pend = rows[placed < 0]
     f = aa_oracle.fulfill_pending_aa(c["req"][pend], len(pend) + 3, c["unit"], c["pool_actual"], c["pool_max"],
                                      c["pool_ignored"], c["over_provision"], c["pod_carries"][pend],
                                      c["pod_matches"][pend], c.get("pool_match"),
@@ -58,8 +66,9 @@ def oracle_of(key):
     return {"placed": placed, "decisions": calls, "used": used, "nc": nc, "nx": nx, "pend": pend, "fulfill": f}
 
 
-def run(engine, c, pend, knobs):
-    """node pass over every pod, then the bin pass over `pend`; returns outputs and launch records of both"""
+def run(engine, c, pend, knobs, pod_idx=None):
+    """node pass over the req rows `pod_idx` (None: every row), then the bin pass over the rows `pend`; returns
+    outputs and launch records of both"""
     try:
         for k, v in knobs.items():
             engine.set_knob(k, v)
@@ -67,7 +76,8 @@ def run(engine, c, pend, knobs):
         d_used = engine.dev(c["used0"], F64)
         d_nc, d_nx = engine.dev(i64(c["node_carries0"]), I64), engine.dev(i64(c["node_matches0"]), I64)
         p, dec = engine.first_fit_nodes_aa(
-            engine.dev(c["req"], F64), None, engine.dev(c["cap_type"], F64), engine.dev(c["node_type"], I32), d_used,
+            engine.dev(c["req"], F64), None if pod_idx is None else engine.dev(pod_idx, I32),
+            engine.dev(c["cap_type"], F64), engine.dev(c["node_type"], I32), d_used,
             engine.dev(i64(c["pod_carries"]), I64), engine.dev(i64(c["pod_matches"]), I64), d_nc, d_nx,
             *((engine.dev(c["pod_class"], U8), engine.dev(i64(c["node_match"]), I64), c["classes"]) if sel else ()))
         node_recs = engine.last_launches()

@@ -74,12 +74,19 @@ def case(base, pa_kind, D):
 
 @functools.lru_cache(maxsize=None)
 def oracle_of(base, pa_kind, D):
-    c = case(base, pa_kind, D)
+    return oracle_of_case(case(base, pa_kind, D))
+
+
+def oracle_of_case(c, pod_idx=None):
+    """the oracle over the req rows `pod_idx` in that order (None: every row); placements and flips are in list
+    positions, and "pend" holds the req rows of the pods left pending, in list order"""
     used, nc, nx, has = c["used0"].copy(), c["node_carries0"].copy(), c["node_matches0"].copy(), c["node_has0"].copy()
+    rows = np.arange(len(c["req"])) if pod_idx is None else np.asarray(pod_idx)
     placed, calls, flips = pa_oracle.first_fit_nodes_pa(
-        c["req"], c["cap_type"], c["node_type"], used, c["pa_requires"], c["pa_self"], c["pa_matches"], has,
-        c["pod_carries"], c["pod_matches"], nc, nx, c.get("node_match"), c.get("pod_class"))
-    pend = np.nonzero(placed < 0)[0]
+        c["req"][rows], c["cap_type"], c["node_type"], used, c["pa_requires"][rows], c["pa_self"][rows],
+        c["pa_matches"][rows], has, c["pod_carries"][rows], c["pod_matches"][rows], nc, nx, c.get("node_match"),
+        None if "pod_class" not in c else c["pod_class"][rows])
+    pend = rows[placed < 0]
     present = int(np.bitwise_or.reduce(has)) if len(has) else 0
     f = pa_oracle.fulfill_pending_pa(c["req"][pend], len(pend) + 3, c["unit"], c["pool_actual"], c["pool_max"],
                                      c["pool_ignored"], c["over_provision"], c["pa_requires"][pend],
@@ -90,7 +97,8 @@ def oracle_of(base, pa_kind, D):
             "pend": pend, "present": present, "fulfill": f}
 
 
-def run(engine, c, pend, present, knobs, with_aa=True):
+def run(engine, c, pend, present, knobs, with_aa=True, pod_idx=None):
+    """the node pass over the req rows `pod_idx` (None: every row), then the bin pass over the rows `pend`"""
     try:
         for k, v in knobs.items():
             engine.set_knob(k, v)
@@ -101,7 +109,8 @@ def run(engine, c, pend, present, knobs, with_aa=True):
         aa = (engine.dev(i64(c["pod_carries"]), I64), engine.dev(i64(c["pod_matches"]), I64), d_nc, d_nx) \
             if with_aa else ()
         p, dec = engine.first_fit_nodes_pa(
-            engine.dev(c["req"], F64), None, engine.dev(c["cap_type"], F64), engine.dev(c["node_type"], I32), d_used,
+            engine.dev(c["req"], F64), None if pod_idx is None else engine.dev(pod_idx, I32),
+            engine.dev(c["cap_type"], F64), engine.dev(c["node_type"], I32), d_used,
             engine.dev(i64(c["pa_requires"]), I64), engine.dev(i64(c["pa_self"]), I64),
             engine.dev(i64(c["pa_matches"]), I64), d_has, *aa,
             **(dict(pod_class=engine.dev(c["pod_class"], U8), node_match=engine.dev(i64(c["node_match"]), I64),

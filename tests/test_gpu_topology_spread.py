@@ -20,6 +20,7 @@ pytestmark = pytest.mark.gpu
 F64, I32, U8, I64 = torch.float64, torch.int32, torch.uint8, torch.int64
 U64 = np.uint64
 INT32_MAX = 2 ** 31 - 1
+MAX_SPREAD_RISES = 4096  # the rises one node pass follows (kMaxSpreadRises in csrc/acsfit.cu)
 # spread overlays: (keys, share of pods with a key, domain nodes per key (0: all), start counts, floor)
 TS_KINDS = {
     "none": (0, 0.0, 0, "zero", "max"),        # no key: the pod-affinity results
@@ -86,14 +87,18 @@ def case(base, ts_kind, pa_kind, D):
     return ts_overlay(pa_overlay(c, pa_kind), ts_kind)
 
 
-def oracle_of_case(c):
+def oracle_of_case(c, pod_idx=None):
+    """the oracle over the req rows `pod_idx` in that order (None: every row); placements, flips and rises are in list
+    positions, and "pend" holds the req rows of the pods left pending, in list order"""
     used, nc, nx, has = c["used0"].copy(), c["node_carries0"].copy(), c["node_matches0"].copy(), c["node_has0"].copy()
     count = c["ts_count0"].copy()
+    rows = np.arange(len(c["req"])) if pod_idx is None else np.asarray(pod_idx)
     placed, calls, flips, rises = ts_oracle.first_fit_nodes_ts(
-        c["req"], c["cap_type"], c["node_type"], used, c["ts_keys"], c["ts_key"], c["ts_skew"], c["ts_matches"],
-        count, c["ts_domain"], c["ts_floor"], c["pa_requires"], c["pa_self"], c["pa_matches"], has,
-        c["pod_carries"], c["pod_matches"], nc, nx, c.get("node_match"), c.get("pod_class"))
-    pend = np.nonzero(placed < 0)[0]
+        c["req"][rows], c["cap_type"], c["node_type"], used, c["ts_keys"], c["ts_key"][rows], c["ts_skew"][rows],
+        c["ts_matches"][rows], count, c["ts_domain"], c["ts_floor"], c["pa_requires"][rows], c["pa_self"][rows],
+        c["pa_matches"][rows], has, c["pod_carries"][rows], c["pod_matches"][rows], nc, nx, c.get("node_match"),
+        None if "pod_class" not in c else c["pod_class"][rows], follow=MAX_SPREAD_RISES)
+    pend = rows[placed < 0]
     present = int(np.bitwise_or.reduce(has)) if len(has) else 0
     f = ts_oracle.fulfill_pending_ts(c["req"][pend], len(pend) + 3, c["unit"], c["pool_actual"], c["pool_max"],
                                      c["pool_ignored"], c["over_provision"], c["ts_keys"], c["ts_key"][pend],
@@ -110,7 +115,8 @@ def oracle_of(base, ts_kind, pa_kind, D):
     return oracle_of_case(case(base, ts_kind, pa_kind, D))
 
 
-def run(engine, c, pend, present, knobs, with_aa=True, with_pa=True):
+def run(engine, c, pend, present, knobs, with_aa=True, with_pa=True, pod_idx=None):
+    """the node pass over the req rows `pod_idx` (None: every row), then the bin pass over the rows `pend`"""
     try:
         for k, v in knobs.items():
             engine.set_knob(k, v)
@@ -124,9 +130,10 @@ def run(engine, c, pend, present, knobs, with_aa=True, with_pa=True):
         pa = tuple(engine.dev(i64(c[k]), I64) for k in ("pa_requires", "pa_self", "pa_matches")) + (d_has,) \
             if with_pa else None
         p, dec = engine.first_fit_nodes_ts(
-            engine.dev(c["req"], F64), None, engine.dev(c["cap_type"], F64), engine.dev(c["node_type"], I32), d_used,
-            c["ts_keys"], engine.dev(c["ts_key"], U8), engine.dev(c["ts_skew"], I32),
-            engine.dev(i64(c["ts_matches"]), I64), d_cnt, engine.dev(i64(c["ts_domain"]), I64), c["ts_floor"],
+            engine.dev(c["req"], F64), None if pod_idx is None else engine.dev(pod_idx, I32),
+            engine.dev(c["cap_type"], F64), engine.dev(c["node_type"], I32), d_used, c["ts_keys"],
+            engine.dev(c["ts_key"], U8), engine.dev(c["ts_skew"], I32), engine.dev(i64(c["ts_matches"]), I64), d_cnt,
+            engine.dev(i64(c["ts_domain"]), I64), c["ts_floor"],
             pa=pa, aa=aa,
             **(dict(pod_class=engine.dev(c["pod_class"], U8), node_match=engine.dev(i64(c["node_match"]), I64),
                     classes=c["classes"]) if sel else {}))
@@ -232,11 +239,11 @@ def test_ts_layouts_match_oracle(eng, name):
     check(eng, name, "rises", "mixed", 0, schedules=("default", "multipass"), scans=(1,))
 
 
-def tile_edge_case():
-    """300 replicas of one group (maxSkew 1) over two roomy nodes: the minimum rises after every second pod, at
-    positions 1, 3, ..., 255 (the last pod of the first 256-pod tile), 257, ..."""
-    P, N, D = 300, 2, 2
-    c = {"req": np.ones((P, D)), "cap_type": np.full((N, D), 1000.0), "node_type": np.arange(N, dtype=np.int32),
+def tile_edge_case(P=300, cap=1000.0):
+    """P replicas of one group (maxSkew 1) over two roomy nodes: the minimum rises after every second pod, at
+    positions 1, 3, ..., 255 (the last pod of the first 256-pod tile), 257, ...; a new node of the pool takes one"""
+    N, D = 2, 2
+    c = {"req": np.ones((P, D)), "cap_type": np.full((N, D), cap), "node_type": np.arange(N, dtype=np.int32),
          "used0": np.zeros((N, D)), "unit": np.full((1, D), 4.0), "pool_actual": np.zeros(1, np.int32),
          "pool_max": np.full(1, 1000, np.int32), "pool_ignored": np.zeros(1, np.uint8), "over_provision": 0,
          "pod_carries": np.zeros(P, U64), "pod_matches": np.zeros(P, U64), "node_carries0": np.zeros(N, U64),

@@ -12,8 +12,9 @@
  *   bin packing : as tests/pa_oracle.c, with spread(p, bin) for min = 0: cnt[key][bin] <= pod_skew[p]; a new bin
  *                 starts with count 0 and so always admits
  * Rises: every time a placement raises a key's minimum, (key, position) is reported, in position order then key order
- * -- the order in which the GPU fixes them.  With every pod_key 0xFF each function is exactly its counterpart in
- * tests/pa_oracle.c (flips included).
+ * -- the order in which the GPU fixes them.  The node pass follows `follow` rises at most (< 0: all): once that many
+ * are reported no key's minimum moves again, as the GPU keeps its levels after its last fixed rise; flips are still
+ * followed.  With every pod_key 0xFF each function is exactly its counterpart in tests/pa_oracle.c (flips included).
  */
 #include <limits.h>
 #include <stdint.h>
@@ -71,7 +72,7 @@ static long long key_min(const int32_t *count, const uint64_t *domain, const int
     return m;
 }
 
-/* rises: room for `max_rises` pairs */
+/* rises: room for `max_rises` pairs; `follow` (< 0: no limit) as above */
 ORACLE_API uint64_t oracle_first_fit_nodes_ts(const double *req, int64_t P, int D, const double *cap_type,
                                               const int32_t *node_type, double *used, int64_t N,
                                               const uint64_t *node_match, const uint8_t *pod_class,
@@ -83,7 +84,7 @@ ORACLE_API uint64_t oracle_first_fit_nodes_ts(const double *req, int64_t P, int 
                                               const uint64_t *ts_matches, int32_t *node_count,
                                               const uint64_t *node_domain, const int32_t *floor, int32_t *placed,
                                               int64_t *flips, int64_t *n_flips, int64_t *rises, int64_t *n_rises,
-                                              int64_t max_rises)
+                                              int64_t max_rises, int64_t follow)
 {
     uint64_t calls = 0, present = 0, selfs = 0;
     long long cur[64];
@@ -122,6 +123,7 @@ ORACLE_API uint64_t oracle_first_fit_nodes_ts(const double *req, int64_t P, int 
             for (int b = 0; b < keys; ++b) {
                 if (!((ts_matches[p] >> b) & 1u)) continue;
                 ++node_count[(size_t)b * N + hit];
+                if (follow >= 0 && *n_rises >= follow) continue;  /* past the last followed rise */
                 const long long m = key_min(node_count, node_domain, floor, N, b);
                 if (m > cur[b] && *n_rises < max_rises) {
                     rises[2 * *n_rises] = b;

@@ -44,9 +44,11 @@ def _pairs(buf, n):
 
 def first_fit_nodes_ts(req, cap_type, node_type, used, keys, pod_key, pod_skew, ts_matches, node_count, node_domain,
                        floor, pod_requires=None, pod_self=None, pod_aff_matches=None, node_has=None, pod_carries=None,
-                       pod_matches=None, node_carries=None, node_matches=None, node_match=None, pod_class=None):
+                       pod_matches=None, node_carries=None, node_matches=None, node_match=None, pod_class=None,
+                       follow=None):
     """mutates `used` and `node_count` (and the affinity node masks when given; contiguous, of their dtypes) in place;
-    returns (placed int32[P], can_fit calls, flips [(signature, position)], rises [(key, position)])"""
+    returns (placed int32[P], can_fit calls, flips [(signature, position)], rises [(key, position)]).  `follow`: the
+    number of rises the pass follows (None: all); after the last one every key keeps its minimum."""
     req, cap_type = _c(req, np.float64), _c(cap_type, np.float64)
     P, D = req.shape
     N = used.shape[0]
@@ -66,7 +68,7 @@ def first_fit_nodes_ts(req, cap_type, node_type, used, keys, pod_key, pod_skew, 
     placed = np.full(P, -1, dtype=np.int32)
     flips = np.zeros(2 * 64, dtype=np.int64)
     n_flips = ctypes.c_int64(0)
-    max_rises = 4 * P + 16
+    max_rises = keys * P + 16  # a pod that several keys select can raise several minimums
     rises = np.zeros(2 * max_rises, dtype=np.int64)
     n_rises = ctypes.c_int64(0)
     calls = lib().oracle_first_fit_nodes_ts(
@@ -75,7 +77,8 @@ def first_fit_nodes_ts(req, cap_type, node_type, used, keys, pod_key, pod_skew, 
         _p(node_matches), _p(pod_requires), _p(pod_self), _p(pod_aff_matches), _p(node_has), ctypes.c_int(keys),
         _p(_c(pod_key, np.uint8)), _p(_c(pod_skew, np.int32)), _p(_c(ts_matches, np.uint64)), _p(node_count),
         _p(_c(node_domain, np.uint64)), _p(_c(np.zeros(0) if floor is None else floor, np.int32)), _p(placed),
-        _p(flips), ctypes.byref(n_flips), _p(rises), ctypes.byref(n_rises), ctypes.c_int64(max_rises))
+        _p(flips), ctypes.byref(n_flips), _p(rises), ctypes.byref(n_rises), ctypes.c_int64(max_rises),
+        ctypes.c_int64(-1 if follow is None else follow))
     return placed, int(calls), _pairs(flips, n_flips.value), _pairs(rises, n_rises.value)
 
 
