@@ -1097,6 +1097,44 @@ static acsfit_status check_req_aligned(acsfit_ctx *ctx, const double *req, const
     return ACSFIT_OK;
 }
 
+// the argument checks every first_fit_nodes* entry point makes before anything else
+static acsfit_status check_first_fit_args(acsfit_ctx *ctx, const char *what, const double *req, int64_t req_rows,
+                                          const void *pod_idx, int64_t P, int D, const void *cap_type,
+                                          const void *node_type, const void *used, int64_t N, const void *placed)
+{
+    if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
+        (P > 0 && (!req || !placed)) || (N > 0 && (!cap_type || !node_type || !used)))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
+    return check_req_aligned(ctx, req, what);
+}
+
+// the argument checks every fulfill_pending* entry point makes before anything else
+static acsfit_status check_fulfill_args(acsfit_ctx *ctx, const char *what, const double *req, int64_t Pp,
+                                        int64_t num_listed, int D, const void *unit, const void *pool_actual,
+                                        const void *pool_max, const void *pool_ignored, int T, const void *new_size,
+                                        const void *units_needed, const void *bins_opened, const void *acc_pool,
+                                        const void *bin_of, const void *unaccounted)
+{
+    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
+        (Pp > 0 && (!req || !acc_pool || !bin_of)) ||
+        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !new_size || !units_needed || !bins_opened)) ||
+        !unaccounted)
+        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
+    if (!pipeline_dims_ok(D))
+        return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
+    return check_req_aligned(ctx, req, what);
+}
+
+// the end of every device-side check: copy its flag word to the host and wait for it
+static acsfit_status flag_to_host(acsfit_ctx *ctx, const int *flag_dev, cudaStream_t st, int *flag)
+{
+    CUDA_TRY(cudaMemcpyAsync(flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return ACSFIT_OK;
+}
+
 static acsfit_status enter(acsfit_ctx *ctx, int D)
 {
     if (!ctx) return ACSFIT_E_INVALID;
@@ -1121,8 +1159,7 @@ static acsfit_status check_domain(acsfit_ctx *ctx, const double *v, int64_t n, i
     domain_kernel<<<grid_for(ctx, n, 256), 256, 0, st>>>(v, n, flag_dev);
     ++ctx->launches;
     int flag = 0;
-    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    TRY(flag_to_host(ctx, flag_dev, st, &flag));
     if (flag) return fail(ctx, ACSFIT_E_DOMAIN, "%s contains a negative or NaN quantity", what);
     return ACSFIT_OK;
 }
@@ -2622,12 +2659,8 @@ extern "C" acsfit_status acsfit_first_fit_nodes(acsfit_ctx *ctx, const double *r
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
-    if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
-        (P > 0 && (!req || !out_placed)) || (N > 0 && (!cap_type || !node_type || !used_inout)))
-        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes: bad arguments");
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
-    TRY(check_req_aligned(ctx, req, "first_fit_nodes"));
+    TRY(check_first_fit_args(ctx, "first_fit_nodes", req, req_rows, pod_idx, P, D, cap_type, node_type, used_inout, N,
+                             out_placed));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + 1024, st));
     ctx->arena_off = 0;
@@ -2649,15 +2682,9 @@ extern "C" acsfit_status acsfit_fulfill_pending(acsfit_ctx *ctx, const double *r
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
-    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
-        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
-        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
-                   !out_bins_opened)) ||
-        !out_unaccounted)
-        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending: bad arguments");
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
-    TRY(check_req_aligned(ctx, req, "fulfill_pending"));
+    TRY(check_fulfill_args(ctx, "fulfill_pending", req, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored,
+                           T, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
+                           out_unaccounted));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + 1024, st));
     ctx->arena_off = 0;
@@ -3339,8 +3366,7 @@ static acsfit_status check_classes(acsfit_ctx *ctx, const uint8_t *pod_class, in
         ++ctx->launches;
     }
     int flag = 0;
-    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    TRY(flag_to_host(ctx, flag_dev, st, &flag));
     CUDA_TRY(cudaGetLastError());
     if (flag & 1) return fail(ctx, ACSFIT_E_INVALID, "%s: a pod_class is >= classes (%d)", what, classes);
     if (flag & 2) return fail(ctx, ACSFIT_E_INVALID, "%s: bit 0 (no selector) must be set in every node mask", what);
@@ -3379,12 +3405,8 @@ extern "C" acsfit_status acsfit_first_fit_nodes_sel(acsfit_ctx *ctx, const doubl
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
-    if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
-        (P > 0 && (!req || !out_placed)) || (N > 0 && (!cap_type || !node_type || !used_inout)))
-        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_sel: bad arguments");
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "first_fit_nodes_sel: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
-    TRY(check_req_aligned(ctx, req, "first_fit_nodes_sel"));
+    TRY(check_first_fit_args(ctx, "first_fit_nodes_sel", req, req_rows, pod_idx, P, D, cap_type, node_type, used_inout,
+                             N, out_placed));
     TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, "first_fit_nodes_sel"));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + 1024, st));
@@ -3410,15 +3432,9 @@ extern "C" acsfit_status acsfit_fulfill_pending_sel(acsfit_ctx *ctx, const doubl
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
-    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
-        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
-        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
-                   !out_bins_opened)) ||
-        !out_unaccounted)
-        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_sel: bad arguments");
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "fulfill_pending_sel: D=%d, need 2/4/8/16 (zero columns are neutral)", D);
-    TRY(check_req_aligned(ctx, req, "fulfill_pending_sel"));
+    TRY(check_fulfill_args(ctx, "fulfill_pending_sel", req, Pp, num_listed, D, unit, pool_actual, pool_max,
+                           pool_ignored, T, out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
+                           out_unaccounted));
     TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, "fulfill_pending_sel"));
     reset_stats(ctx);
     TRY(arena_reserve(ctx, fulfill_scratch(Pp, T, D) + rank_scratch(Pp, D) + 1024, st));
@@ -3487,8 +3503,7 @@ static acsfit_status check_pa_host(acsfit_ctx *ctx, const acsfit_pod_affinity *p
                                                               rows, flag_dev);
     ++ctx->launches;
     int flag = 0;
-    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    TRY(flag_to_host(ctx, flag_dev, st, &flag));
     CUDA_TRY(cudaGetLastError());
     if (flag & 4) return fail(ctx, ACSFIT_E_INVALID, "%s: a pod_requires has more than one bit, or pod_self is not inside it", what);
     return ACSFIT_OK;
@@ -3525,8 +3540,7 @@ static acsfit_status check_ts_host(acsfit_ctx *ctx, const acsfit_topology_spread
         ts->node_count, counts, flag_dev);
     ++ctx->launches;
     int flag = 0;
-    CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    TRY(flag_to_host(ctx, flag_dev, st, &flag));
     CUDA_TRY(cudaGetLastError());
     if (flag & 8)
         return fail(ctx, ACSFIT_E_INVALID, "%s: a pod_key is >= keys, a pod_skew is negative, or a pod_matches names a "
@@ -3555,29 +3569,20 @@ static acsfit_status first_fit_nodes_aa_pa(acsfit_ctx *ctx, const double *req, i
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
-    if (P < 0 || N < 0 || req_rows < 0 || P > INT32_MAX || N > INT32_MAX || (!pod_idx && P > req_rows) ||
-        (P > 0 && (!req || !out_placed)) || (N > 0 && (!cap_type || !node_type || !used_inout)))
-        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
-    TRY(check_req_aligned(ctx, req, what));
+    TRY(check_first_fit_args(ctx, what, req, req_rows, pod_idx, P, D, cap_type, node_type, used_inout, N, out_placed));
     if ((!pa && !ts) || aa) TRY(check_aa_host(ctx, aa, req_rows, N, what));
     if (sel) TRY(check_selectors_host(ctx, sel, req_rows, N, 0, kSelNodes, what));
     if (ts && ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: topology spread is not supported in cluster mode", what);
     reset_stats(ctx);
     // without selectors: class 0 for every row and all-ones node masks, from the arena
     const size_t trivial = sel ? 0 : align_up((size_t)req_rows, 256) + sizeof(uint64_t) * (size_t)N + 512;
-    // pod affinity: zero anti-affinity masks without `aa`, the needs, and the saved node state of a rerun
-    const size_t pa_bytes = !pa ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)(req_rows + N) + 256) +
-                                          sizeof(uint64_t) * (size_t)P + sizeof(double) * (size_t)N * D +
-                                          sizeof(uint64_t) * 3 * (size_t)N + 2048;
-    // topology spread: zero pod-affinity masks without `pa` (and then the pod-affinity scratch), the limits, the
-    // saved counts of a rerun
-    const size_t pa_n = ts && !pa ? (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)(req_rows + N) + 256) +
-                                        sizeof(uint64_t) * (size_t)P + sizeof(double) * (size_t)N * D +
-                                        sizeof(uint64_t) * 3 * (size_t)N + 2048
-                                  : 0;
-    const size_t ts_bytes = !ts ? 0 : pa_n + (pa ? 0 : sizeof(uint64_t) * (size_t)(3 * req_rows + N) + 256) +
+    // pod affinity, which topology spread runs on too (with zero masks without `pa`): zero anti-affinity masks
+    // without `aa`, the needs, and the saved node state of a rerun
+    const size_t pa_bytes = !pa && !ts ? 0 : (aa ? 0 : sizeof(uint64_t) * 2 * (size_t)(req_rows + N) + 256) +
+                                                 sizeof(uint64_t) * (size_t)P + sizeof(double) * (size_t)N * D +
+                                                 sizeof(uint64_t) * 3 * (size_t)N + 2048;
+    // topology spread: zero pod-affinity masks without `pa`, the limits, the saved counts of a rerun
+    const size_t ts_bytes = !ts ? 0 : (pa ? 0 : sizeof(uint64_t) * (size_t)(3 * req_rows + N) + 256) +
                                           ts_scratch(P) + sizeof(int32_t) * (size_t)N * std::max(0, ts->keys) + 256;
     TRY(arena_reserve(ctx, first_fit_scratch(ctx, P, N) + rank_scratch(req_rows, D) + trivial + pa_bytes + ts_bytes + 1024, st));
     ctx->arena_off = 0;
@@ -3649,15 +3654,9 @@ static acsfit_status fulfill_pending_aa_pa(acsfit_ctx *ctx, const double *req, i
 {
     TRY(enter(ctx, D));
     cudaStream_t st = (cudaStream_t)stream;
-    if (Pp < 0 || Pp > INT32_MAX || num_listed < Pp || T < 0 || T > ACSFIT_MAX_POOLS ||
-        (Pp > 0 && (!req || !out_acc_pool || !out_bin_of)) ||
-        (T > 0 && (!unit || !pool_actual || !pool_max || !pool_ignored || !out_new_size || !out_units_needed ||
-                   !out_bins_opened)) ||
-        !out_unaccounted)
-        return fail(ctx, ACSFIT_E_INVALID, "%s: bad arguments", what);
-    if (!pipeline_dims_ok(D))
-        return fail(ctx, ACSFIT_E_INVALID, "%s: D=%d, need 2/4/8/16 (zero columns are neutral)", what, D);
-    TRY(check_req_aligned(ctx, req, what));
+    TRY(check_fulfill_args(ctx, what, req, Pp, num_listed, D, unit, pool_actual, pool_max, pool_ignored, T,
+                           out_new_size, out_units_needed, out_bins_opened, out_acc_pool, out_bin_of,
+                           out_unaccounted));
     if ((!pa && !ts) || aa) TRY(check_aa_host(ctx, aa, Pp, 0, what));
     if (sel) TRY(check_selectors_host(ctx, sel, Pp, 0, T, kSelPoolsOrdered, what));
     if (ts && ctx->world > 1) return fail(ctx, ACSFIT_E_INVALID, "%s: topology spread is not supported in cluster mode", what);

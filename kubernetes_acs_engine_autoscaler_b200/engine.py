@@ -38,6 +38,44 @@ def _np(a, dtype):
     return np.ascontiguousarray(a, dtype=dtype)
 
 
+def _ref(s):
+    """pointer to a ctypes object (a rule struct, or a value the library writes back), NULL for None"""
+    return None if s is None else ctypes.cast(ctypes.byref(s), ctypes.c_void_p)
+
+
+def _pools(D, units, pool_actual, pool_max, pool_ignored):
+    """host pool arguments as the C ABI takes them: each unit table as float64 [T, D], then the per-pool arrays"""
+    return tuple(_np(u, np.float64).reshape(-1, D) for u in units) + (
+        _np(pool_actual, np.int32), _np(pool_max, np.int32), _np(pool_ignored, np.uint8))
+
+
+def _fulfill_result(out):
+    """the result dict of a fulfill_pending* call from the outputs of Engine._fulfill_out"""
+    return dict(out, num_unaccounted=int(out["num_unaccounted"].value), evals=int(out["evals"].value))
+
+
+def _host_pod_outputs(P):
+    return {"feasible": np.empty(P, dtype=np.uint8), "placed": np.empty(P, dtype=np.int32),
+            "acc_pool": np.empty(P, dtype=np.int32)}
+
+
+def _scale_up_out(out, T):
+    """(result dict, its pointer arguments in ABI order, counters) of a scale_up* call around `out`, the per-pod
+    arrays feasible / placed / acc_pool"""
+    res = dict(out)
+    for k in ("new_size", "units_needed", "bins_opened"):
+        res[k] = np.zeros(T, dtype=np.int64)
+    counters = np.zeros(4, dtype=np.uint64)
+    args = [_ptr(res[k]) for k in ("feasible", "placed", "new_size", "units_needed", "bins_opened", "acc_pool")]
+    return res, args + [_ptr(counters)], counters
+
+
+def _scale_up_result(res, counters):
+    res.update({"n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
+                "num_unaccounted": int(counters[2]), "decisions": int(counters[3])})
+    return res
+
+
 class Engine(object):
     """one acsfit context on one GPU (one per process / per rank)."""
 
@@ -84,6 +122,34 @@ class Engine(object):
     def empty(self, shape, dtype):
         return torch.empty(shape, dtype=dtype, device=self.device)
 
+    def _first_fit_out(self, req, pod_idx, used):
+        """(rows, D, P, N, placed, decisions) of a first_fit_nodes* call"""
+        rows, D = req.shape
+        P = rows if pod_idx is None else pod_idx.shape[0]
+        return rows, D, P, used.shape[0], self.empty((P,), torch.int32), \
+            torch.zeros(1, dtype=torch.int64, device=self.device)
+
+    def _fulfill_out(self, Pp, T):
+        """(outputs, their pointer arguments in ABI order) of a fulfill_pending* call; see _fulfill_result"""
+        out = {"new_size": np.zeros(T, dtype=np.int64), "units_needed": np.zeros(T, dtype=np.int64),
+               "bins_opened": np.zeros(T, dtype=np.int64), "acc_pool": self.empty((Pp,), torch.int32),
+               "bin_of": self.empty((Pp,), torch.int32), "num_unaccounted": ctypes.c_int64(0),
+               "evals": ctypes.c_uint64(0)}
+        args = [_ptr(out[k]) for k in ("new_size", "units_needed", "bins_opened", "acc_pool", "bin_of")]
+        return out, args + [_ref(out["num_unaccounted"]), _ref(out["evals"])]
+
+    def _pod_outputs(self, P):
+        return {"feasible": self.empty((P,), torch.uint8), "placed": self.empty((P,), torch.int32),
+                "acc_pool": self.empty((P,), torch.int32)}
+
+    def _pairs(self, fn):
+        """the (a, b) pairs a two-call test hook reports: the count first, then the pairs"""
+        n = ctypes.c_int64(0)
+        self._check(fn(self._ctx, _ref(n), None))
+        out = np.zeros(2 * n.value, dtype=np.int64)
+        self._check(fn(self._ctx, _ref(n), _ptr(out)))
+        return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(n.value)]
+
     def set_timing(self, enabled):
         self._check(self._lib.acsfit_ctx_set_timing(self._ctx, 1 if enabled else 0))
 
@@ -122,7 +188,7 @@ class Engine(object):
 
     def cluster_last_plan(self):
         v = [ctypes.c_int() for _ in range(4)]
-        self._check(self._lib.acsfit_cluster_last_plan(self._ctx, *[ctypes.cast(ctypes.byref(x), ctypes.c_void_p) for x in v]))
+        self._check(self._lib.acsfit_cluster_last_plan(self._ctx, *[_ref(x) for x in v]))
         return {"stage_nodes": v[0].value, "stages": v[1].value, "pod_blocks": v[2].value, "resident": v[3].value}
 
     @property
@@ -143,10 +209,9 @@ class Engine(object):
         (keys: _native.LAUNCH_FIELDS; "pass" 0 = nodes / 1 = bins, "RW" 0 = float64 scan, "form" 1 = streaming)."""
         nf = len(_native.LAUNCH_FIELDS)
         n = ctypes.c_int(0)
-        self._check(self._lib.acsfit_last_launches(self._ctx, None, 0, ctypes.cast(ctypes.byref(n), ctypes.c_void_p)))
+        self._check(self._lib.acsfit_last_launches(self._ctx, None, 0, _ref(n)))
         out = np.zeros((max(n.value, 1), nf), dtype=np.int32)
-        self._check(self._lib.acsfit_last_launches(self._ctx, _ptr(out), n.value,
-                                                   ctypes.cast(ctypes.byref(n), ctypes.c_void_p)))
+        self._check(self._lib.acsfit_last_launches(self._ctx, _ptr(out), n.value, _ref(n)))
         return [dict(zip(_native.LAUNCH_FIELDS, (int(v) for v in row))) for row in out[:n.value]]
 
     def last_scan_launch(self):
@@ -160,7 +225,7 @@ class Engine(object):
         """test hook: pods the candidate scan of the last call's selector node passes handed to the resolver (summed over
         tiles and stages; a pod counts in a stage only when some node there fits it AND matches its selector class)."""
         out = ctypes.c_uint64(0)
-        self._check(self._lib.acsfit_last_sel_hits(self._ctx, ctypes.cast(ctypes.byref(out), ctypes.c_void_p)))
+        self._check(self._lib.acsfit_last_sel_hits(self._ctx, _ref(out)))
         return int(out.value)
 
     def last_bin_retirement(self):
@@ -172,20 +237,14 @@ class Engine(object):
 
     def last_affinity_reruns(self):
         """test hook: the (signature, position) flips the last pod-affinity call fixed, one per pass it ran again."""
-        n = ctypes.c_int64(0)
-        self._check(self._lib.acsfit_last_affinity_reruns(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p), None))
-        out = np.zeros(2 * n.value, dtype=np.int64)
-        self._check(self._lib.acsfit_last_affinity_reruns(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p),
-                                                          _ptr(out)))
-        return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(n.value)]
+        return self._pairs(self._lib.acsfit_last_affinity_reruns)
 
     def debug_profile(self, enabled=True):
         """developer probe: per-stage clock64 totals [stages, 8] of the last pipeline launch
         (wait, load, scan, resolve, publish, refresh, hits, tiles)."""
         out = np.zeros((4096, 8), dtype=np.uint64)
         n = ctypes.c_int(0)
-        self._check(self._lib.acsfit_debug_profile(self._ctx, 1 if enabled else 0, _ptr(out), 4096,
-                                                   ctypes.cast(ctypes.byref(n), ctypes.c_void_p)))
+        self._check(self._lib.acsfit_debug_profile(self._ctx, 1 if enabled else 0, _ptr(out), 4096, _ref(n)))
         return out[:n.value]
 
     def debug_trace(self, stage, tiles=8192):
@@ -215,11 +274,7 @@ class Engine(object):
     def first_fit_nodes(self, req, pod_idx, cap_type, node_type, used):
         """Cluster.get_pending_pods (cluster.py:184-204). Returns (placed int32[P] device,
         decisions int64[1] device); `used` is updated in place."""
-        rows, D = req.shape
-        P = rows if pod_idx is None else pod_idx.shape[0]
-        N = used.shape[0]
-        placed = self.empty((P,), torch.int32)
-        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
+        rows, D, P, N, placed, decisions = self._first_fit_out(req, pod_idx, used)
         self._check(self._lib.acsfit_first_fit_nodes(self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type),
                                                      _ptr(node_type), _ptr(used), N, _ptr(placed), _ptr(decisions),
                                                      self._stream()))
@@ -228,26 +283,13 @@ class Engine(object):
     def fulfill_pending(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision):
         """Scaler.fulfill_pending up to scaler.py:177. req [Pp,D] device; pool arrays host (visiting order)."""
         Pp, D = req.shape
-        unit = _np(unit, np.float64).reshape(-1, D)
+        unit, pool_actual, pool_max, pool_ignored = _pools(D, [unit], pool_actual, pool_max, pool_ignored)
         T = unit.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        acc_pool = self.empty((Pp,), torch.int32)
-        bin_of = self.empty((Pp,), torch.int32)
-        unacc = ctypes.c_int64(0)
-        evals = ctypes.c_uint64(0)
+        out, outs = self._fulfill_out(Pp, T)
         self._check(self._lib.acsfit_fulfill_pending(
             self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened),
-            _ptr(acc_pool), _ptr(bin_of), ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p),
-            ctypes.cast(ctypes.byref(evals), ctypes.c_void_p), self._stream()))
-        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
-                "evals": int(evals.value)}
+            _ptr(pool_ignored), T, int(over_provision), *outs, self._stream()))
+        return _fulfill_result(out)
 
     def node_states(self, row_ptr, run_idx, req_run, flags_run, cap_type, node_type, node_flags, node_age,
                     any_pending, idle_thresholds):
@@ -319,8 +361,7 @@ class Engine(object):
         self._check(self._lib.acsfit_pending_admit_ts(self._ctx, _ptr(row_ptr), _ptr(run_carries), _ptr(run_matches),
                                                       _ptr(run_has), N, _ptr(node_match), _ptr(sig_class),
                                                       _ptr(sig_carries), _ptr(sig_matches), _ptr(sig_need),
-                                                      _ptr(sig_key), _ptr(sig_skew), U,
-                                                      ctypes.cast(ctypes.byref(ts), ctypes.c_void_p), _ptr(node_flags),
+                                                      _ptr(sig_key), _ptr(sig_skew), U, _ref(ts), _ptr(node_flags),
                                                       self._stream()))
         return node_flags
 
@@ -341,28 +382,15 @@ class Engine(object):
         """fused get_pods_to_schedule + get_pending_pods + fulfill_pending on device buffers."""
         P, D = req.shape
         N = used.shape[0]
-        unit_all = _np(unit_all, np.float64).reshape(-1, D)
-        unit_ordered = _np(unit_ordered, np.float64).reshape(-1, D)
+        unit_all, unit_ordered, pool_actual, pool_max, pool_ignored = _pools(D, [unit_all, unit_ordered], pool_actual,
+                                                                             pool_max, pool_ignored)
         T = unit_all.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        feasible = self.empty((P,), torch.uint8)
-        placed = self.empty((P,), torch.int32)
-        acc_pool = self.empty((P,), torch.int32)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        counters = np.zeros(4, dtype=np.uint64)
+        res, outs, counters = _scale_up_out(self._pod_outputs(P), T)
         self._check(self._lib.acsfit_scale_up(
             self._ctx, _ptr(req), P, D, _ptr(unit_all), _ptr(unit_ordered), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), _ptr(node_type), _ptr(used), N,
-            _ptr(feasible), _ptr(placed), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool),
-            _ptr(counters), self._stream()))
-        return {"feasible": feasible, "placed": placed, "acc_pool": acc_pool, "new_size": new_size,
-                "units_needed": units_needed, "bins_opened": bins_opened,
-                "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
-                "num_unaccounted": int(counters[2]), "decisions": int(counters[3])}
+            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), _ptr(node_type), _ptr(used), N, *outs,
+            self._stream()))
+        return _scale_up_result(res, counters)
 
     # ------------------------------------------------------------------ node selectors (include/acsfit.h)
     @staticmethod
@@ -376,6 +404,11 @@ class Engine(object):
         sel = _native.Selectors(*[None if a is None else _ptr(a).value for a in keep], int(classes))
         return sel, keep
 
+    @staticmethod
+    def _selectors_if(classes, pod_class, **masks):
+        """_selectors when pod_class is given (the rule forms take selectors as an option), else (None, None)"""
+        return (None, None) if pod_class is None else Engine._selectors(classes, pod_class, **masks)
+
     def feasible_mask_sel(self, req, unit, pod_class, pool_match, classes):
         """feasible_mask with node selectors: pod_class uint8 [P] device, pool_match uint64 [T] host
         (agent_pools order)."""
@@ -384,22 +417,17 @@ class Engine(object):
         mask = self.empty((P,), torch.uint8)
         evals = torch.zeros(1, dtype=torch.int64, device=self.device)
         sel, keep = self._selectors(classes, pod_class=pod_class, pool_match_all=pool_match)
-        self._check(self._lib.acsfit_feasible_mask_sel(self._ctx, _ptr(req), P, D, _ptr(unit), T,
-                                                       ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(mask),
-                                                       _ptr(evals), self._stream()))
+        self._check(self._lib.acsfit_feasible_mask_sel(self._ctx, _ptr(req), P, D, _ptr(unit), T, _ref(sel),
+                                                       _ptr(mask), _ptr(evals), self._stream()))
         return mask, evals
 
     def first_fit_nodes_sel(self, req, pod_idx, cap_type, node_type, used, pod_class, node_match, classes):
         """first_fit_nodes with node selectors: pod_class uint8 [req rows] device, node_match uint64 [N] device."""
-        rows, D = req.shape
-        P = rows if pod_idx is None else pod_idx.shape[0]
-        N = used.shape[0]
-        placed = self.empty((P,), torch.int32)
-        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
+        rows, D, P, N, placed, decisions = self._first_fit_out(req, pod_idx, used)
         sel, keep = self._selectors(classes, pod_class=pod_class, node_match=node_match)
         self._check(self._lib.acsfit_first_fit_nodes_sel(
             self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
-            ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(placed), _ptr(decisions), self._stream()))
+            _ref(sel), _ptr(placed), _ptr(decisions), self._stream()))
         return placed, decisions
 
     def fulfill_pending_sel(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision,
@@ -407,57 +435,30 @@ class Engine(object):
         """fulfill_pending with node selectors: pod_class uint8 [Pp] device, pool_match uint64 [T] host (visiting
         order, like every other pool array here)."""
         Pp, D = req.shape
-        unit = _np(unit, np.float64).reshape(-1, D)
+        unit, pool_actual, pool_max, pool_ignored = _pools(D, [unit], pool_actual, pool_max, pool_ignored)
         T = unit.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        acc_pool = self.empty((Pp,), torch.int32)
-        bin_of = self.empty((Pp,), torch.int32)
-        unacc = ctypes.c_int64(0)
-        evals = ctypes.c_uint64(0)
+        out, outs = self._fulfill_out(Pp, T)
         sel, keep = self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
         self._check(self._lib.acsfit_fulfill_pending_sel(
             self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
-            _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(bin_of),
-            ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p), ctypes.cast(ctypes.byref(evals), ctypes.c_void_p),
-            self._stream()))
-        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
-                "evals": int(evals.value)}
+            _ptr(pool_ignored), T, int(over_provision), _ref(sel), *outs, self._stream()))
+        return _fulfill_result(out)
 
     def scale_up_sel(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,
                      cap_type, node_type, used, pod_class, node_match, pool_match_all, pool_match_ordered, classes):
         """scale_up with node selectors: pod_class uint8 [P] / node_match uint64 [N] device, the pool masks host."""
         P, D = req.shape
         N = used.shape[0]
-        unit_all = _np(unit_all, np.float64).reshape(-1, D)
-        unit_ordered = _np(unit_ordered, np.float64).reshape(-1, D)
+        unit_all, unit_ordered, pool_actual, pool_max, pool_ignored = _pools(D, [unit_all, unit_ordered], pool_actual,
+                                                                             pool_max, pool_ignored)
         T = unit_all.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        feasible = self.empty((P,), torch.uint8)
-        placed = self.empty((P,), torch.int32)
-        acc_pool = self.empty((P,), torch.int32)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        counters = np.zeros(4, dtype=np.uint64)
+        res, outs, counters = _scale_up_out(self._pod_outputs(P), T)
         sel, keep = self._selectors(classes, pod_class, node_match, pool_match_all, pool_match_ordered)
         self._check(self._lib.acsfit_scale_up_sel(
             self._ctx, _ptr(req), P, D, _ptr(unit_all), _ptr(unit_ordered), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), _ptr(node_type), _ptr(used), N,
-            ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(feasible), _ptr(placed), _ptr(new_size),
-            _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(counters), self._stream()))
-        return {"feasible": feasible, "placed": placed, "acc_pool": acc_pool, "new_size": new_size,
-                "units_needed": units_needed, "bins_opened": bins_opened,
-                "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
-                "num_unaccounted": int(counters[2]), "decisions": int(counters[3])}
+            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), _ptr(node_type), _ptr(used), N, _ref(sel),
+            *outs, self._stream()))
+        return _scale_up_result(res, counters)
 
     def scale_up_sel_host(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,
                           cap_type, node_type, used, pod_class, node_match, pool_match_all, pool_match_ordered,
@@ -470,30 +471,17 @@ class Engine(object):
         node_type = _np(node_type, np.int32)
         assert isinstance(used, np.ndarray) and used.dtype == np.float64 and used.flags.c_contiguous
         N = used.shape[0]
-        unit_all = _np(unit_all, np.float64).reshape(-1, D)
-        unit_ordered = _np(unit_ordered, np.float64).reshape(-1, D)
+        unit_all, unit_ordered, pool_actual, pool_max, pool_ignored = _pools(D, [unit_all, unit_ordered], pool_actual,
+                                                                             pool_max, pool_ignored)
         T = unit_all.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        out = {"feasible": np.empty(P, dtype=np.uint8), "placed": np.empty(P, dtype=np.int32),
-               "acc_pool": np.empty(P, dtype=np.int32)}
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        counters = np.zeros(4, dtype=np.uint64)
+        res, outs, counters = _scale_up_out(_host_pod_outputs(P), T)
         sel, keep = self._selectors(classes, _np(pod_class, np.uint8), _np(node_match, np.uint64), pool_match_all,
                                     pool_match_ordered)
         self._check(self._lib.acsfit_scale_up_sel_host(
             self._ctx, _ptr(req), P, D, _ptr(unit_all), _ptr(unit_ordered), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), K, _ptr(node_type), _ptr(used), N,
-            ctypes.cast(ctypes.byref(sel), ctypes.c_void_p), _ptr(out["feasible"]), _ptr(out["placed"]),
-            _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(out["acc_pool"]), _ptr(counters)))
-        res = dict(out)
-        res.update({"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                    "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
-                    "num_unaccounted": int(counters[2]), "decisions": int(counters[3])})
-        return res
+            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), K, _ptr(node_type), _ptr(used), N, _ref(sel),
+            *outs))
+        return _scale_up_result(res, counters)
 
     # ------------------------------------------------------------------ pod anti-affinity (include/acsfit.h)
     @staticmethod
@@ -503,23 +491,22 @@ class Engine(object):
         aa = _native.AntiAffinity(*[None if a is None else _ptr(a).value for a in keep])
         return aa, keep
 
+    @staticmethod
+    def _anti_affinity_if(pod_carries, *masks):
+        """_anti_affinity when pod_carries is given (the later rule forms take it as an option), else (None, None)"""
+        return (None, None) if pod_carries is None else Engine._anti_affinity(pod_carries, *masks)
+
     def first_fit_nodes_aa(self, req, pod_idx, cap_type, node_type, used, pod_carries, pod_matches, node_carries,
                            node_matches, pod_class=None, node_match=None, classes=1):
         """first_fit_nodes with required pod anti-affinity: pod_carries / pod_matches uint64 [req rows] device (stored
         as int64), node_carries / node_matches uint64 [N] device, updated in place like `used`.  pod_class /
         node_match (both or neither): node selectors as in first_fit_nodes_sel."""
-        rows, D = req.shape
-        P = rows if pod_idx is None else pod_idx.shape[0]
-        N = used.shape[0]
-        placed = self.empty((P,), torch.int32)
-        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
-        sel, keep_s = (None, None) if pod_class is None else \
-            self._selectors(classes, pod_class=pod_class, node_match=node_match)
+        rows, D, P, N, placed, decisions = self._first_fit_out(req, pod_idx, used)
+        sel, keep_s = self._selectors_if(classes, pod_class, node_match=node_match)
         aa, keep_a = self._anti_affinity(pod_carries, pod_matches, node_carries, node_matches)
         self._check(self._lib.acsfit_first_fit_nodes_aa(
             self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
-            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
-            ctypes.cast(ctypes.byref(aa), ctypes.c_void_p), _ptr(placed), _ptr(decisions), self._stream()))
+            _ref(sel), _ref(aa), _ptr(placed), _ptr(decisions), self._stream()))
         return placed, decisions
 
     def fulfill_pending_aa(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision,
@@ -527,41 +514,20 @@ class Engine(object):
         """fulfill_pending with required pod anti-affinity in the bins: pod_carries / pod_matches uint64 [Pp] device
         (stored as int64).  pod_class / pool_match (both or neither): node selectors as in fulfill_pending_sel."""
         Pp, D = req.shape
-        unit = _np(unit, np.float64).reshape(-1, D)
+        unit, pool_actual, pool_max, pool_ignored = _pools(D, [unit], pool_actual, pool_max, pool_ignored)
         T = unit.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        acc_pool = self.empty((Pp,), torch.int32)
-        bin_of = self.empty((Pp,), torch.int32)
-        unacc = ctypes.c_int64(0)
-        evals = ctypes.c_uint64(0)
-        sel, keep_s = (None, None) if pod_class is None else \
-            self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
+        out, outs = self._fulfill_out(Pp, T)
+        sel, keep_s = self._selectors_if(classes, pod_class, pool_match_ordered=pool_match)
         aa, keep_a = self._anti_affinity(pod_carries, pod_matches)
         self._check(self._lib.acsfit_fulfill_pending_aa(
             self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision),
-            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
-            ctypes.cast(ctypes.byref(aa), ctypes.c_void_p), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened),
-            _ptr(acc_pool), _ptr(bin_of), ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p),
-            ctypes.cast(ctypes.byref(evals), ctypes.c_void_p), self._stream()))
-        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
-                "evals": int(evals.value)}
+            _ptr(pool_ignored), T, int(over_provision), _ref(sel), _ref(aa), *outs, self._stream()))
+        return _fulfill_result(out)
 
     # ------------------------------------------------------------------ topology spread (include/acsfit.h)
     def last_spread_rises(self):
         """test hook: the (key, position) rises the last topology-spread call fixed, one per pass it ran again."""
-        n = ctypes.c_int64(0)
-        self._check(self._lib.acsfit_last_spread_rises(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p), None))
-        out = np.zeros(2 * n.value, dtype=np.int64)
-        self._check(self._lib.acsfit_last_spread_rises(self._ctx, ctypes.cast(ctypes.byref(n), ctypes.c_void_p),
-                                                       _ptr(out)))
-        return [(int(out[2 * k]), int(out[2 * k + 1])) for k in range(n.value)]
+        return self._pairs(self._lib.acsfit_last_spread_rises)
 
     @staticmethod
     def _spread(keys, pod_key, pod_skew, pod_matches, node_count=None, node_domain=None, floor=None):
@@ -578,20 +544,14 @@ class Engine(object):
         floor int32 [keys] host; node_count is updated in place like `used`.  `pa` (pod_requires, pod_self,
         pod_matches, node_has) and `aa` (pod_carries, pod_matches, node_carries, node_matches) device tuples or None;
         pod_class / node_match (both or neither) as in first_fit_nodes_aa."""
-        rows, D = req.shape
-        P = rows if pod_idx is None else pod_idx.shape[0]
-        N = used.shape[0]
-        placed = self.empty((P,), torch.int32)
-        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
-        sel, keep_s = (None, None) if pod_class is None else \
-            self._selectors(classes, pod_class=pod_class, node_match=node_match)
-        a, keep_a = (None, None) if aa is None else self._anti_affinity(*aa)
+        rows, D, P, N, placed, decisions = self._first_fit_out(req, pod_idx, used)
+        sel, keep_s = self._selectors_if(classes, pod_class, node_match=node_match)
+        a, keep_a = self._anti_affinity_if(*(aa or (None,)))
         p = None if pa is None else _native.PodAffinity(*[_ptr(t).value for t in pa])
         ts, keep_t = self._spread(keys, pod_key, pod_skew, pod_matches, node_count, node_domain, floor)
-        ref = lambda s: None if s is None else ctypes.cast(ctypes.byref(s), ctypes.c_void_p)  # noqa: E731
         self._check(self._lib.acsfit_first_fit_nodes_ts(
             self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
-            ref(sel), ref(a), ref(p), ref(ts), _ptr(placed), _ptr(decisions), self._stream()))
+            _ref(sel), _ref(a), _ref(p), _ref(ts), _ptr(placed), _ptr(decisions), self._stream()))
         return placed, decisions
 
     def fulfill_pending_ts(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision, keys,
@@ -601,33 +561,18 @@ class Engine(object):
         in first_fit_nodes_ts.  `pa` (pod_requires, pod_self, pod_matches) and `aa` (pod_carries, pod_matches) device
         tuples or None; `present` and pod_class / pool_match as in fulfill_pending_pa."""
         Pp, D = req.shape
-        unit = _np(unit, np.float64).reshape(-1, D)
+        unit, pool_actual, pool_max, pool_ignored = _pools(D, [unit], pool_actual, pool_max, pool_ignored)
         T = unit.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        acc_pool = self.empty((Pp,), torch.int32)
-        bin_of = self.empty((Pp,), torch.int32)
-        unacc = ctypes.c_int64(0)
-        evals = ctypes.c_uint64(0)
-        sel, keep_s = (None, None) if pod_class is None else \
-            self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
-        a, keep_a = (None, None) if aa is None else self._anti_affinity(*aa)
+        out, outs = self._fulfill_out(Pp, T)
+        sel, keep_s = self._selectors_if(classes, pod_class, pool_match_ordered=pool_match)
+        a, keep_a = self._anti_affinity_if(*(aa or (None,)))
         p = None if pa is None else _native.PodAffinity(*[_ptr(t).value for t in pa], None)
         ts, keep_t = self._spread(keys, pod_key, pod_skew, pod_matches)
-        ref = lambda s: None if s is None else ctypes.cast(ctypes.byref(s), ctypes.c_void_p)  # noqa: E731
         self._check(self._lib.acsfit_fulfill_pending_ts(
             self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), ref(sel), ref(a), ref(p), int(present) & 0xFFFFFFFFFFFFFFFF,
-            ref(ts), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(bin_of),
-            ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p), ctypes.cast(ctypes.byref(evals), ctypes.c_void_p),
-            self._stream()))
-        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
-                "evals": int(evals.value)}
+            _ptr(pool_ignored), T, int(over_provision), _ref(sel), _ref(a), _ref(p), int(present) & 0xFFFFFFFFFFFFFFFF,
+            _ref(ts), *outs, self._stream()))
+        return _fulfill_result(out)
 
     # ------------------------------------------------------------------ pod affinity (include/acsfit.h)
     def first_fit_nodes_pa(self, req, pod_idx, cap_type, node_type, used, pod_requires, pod_self, pod_matches, node_has,
@@ -636,22 +581,14 @@ class Engine(object):
         """first_fit_nodes with required pod affinity: pod_requires / pod_self / pod_matches uint64 [req rows] device
         (stored as int64), node_has uint64 [N] device, updated in place like `used`.  The anti-affinity masks (all four
         or none) and pod_class / node_match (both or neither) as in first_fit_nodes_aa."""
-        rows, D = req.shape
-        P = rows if pod_idx is None else pod_idx.shape[0]
-        N = used.shape[0]
-        placed = self.empty((P,), torch.int32)
-        decisions = torch.zeros(1, dtype=torch.int64, device=self.device)
-        sel, keep_s = (None, None) if pod_class is None else \
-            self._selectors(classes, pod_class=pod_class, node_match=node_match)
-        aa, keep_a = (None, None) if pod_carries is None else \
-            self._anti_affinity(pod_carries, pod_matches_aa, node_carries, node_matches)
+        rows, D, P, N, placed, decisions = self._first_fit_out(req, pod_idx, used)
+        sel, keep_s = self._selectors_if(classes, pod_class, node_match=node_match)
+        aa, keep_a = self._anti_affinity_if(pod_carries, pod_matches_aa, node_carries, node_matches)
         keep_p = [pod_requires, pod_self, pod_matches, node_has]
         pa = _native.PodAffinity(*[None if a is None else _ptr(a).value for a in keep_p])
         self._check(self._lib.acsfit_first_fit_nodes_pa(
             self._ctx, _ptr(req), rows, _ptr(pod_idx), P, D, _ptr(cap_type), _ptr(node_type), _ptr(used), N,
-            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
-            None if aa is None else ctypes.cast(ctypes.byref(aa), ctypes.c_void_p),
-            ctypes.cast(ctypes.byref(pa), ctypes.c_void_p), _ptr(placed), _ptr(decisions), self._stream()))
+            _ref(sel), _ref(aa), _ref(pa), _ptr(placed), _ptr(decisions), self._stream()))
         return placed, decisions
 
     def fulfill_pending_pa(self, req, num_listed, unit, pool_actual, pool_max, pool_ignored, over_provision,
@@ -661,35 +598,18 @@ class Engine(object):
         device (stored as int64); `present` the signatures the nodes already hold (0: only pods this call places
         count).  The anti-affinity masks (both or neither) and pod_class / pool_match as in fulfill_pending_aa."""
         Pp, D = req.shape
-        unit = _np(unit, np.float64).reshape(-1, D)
+        unit, pool_actual, pool_max, pool_ignored = _pools(D, [unit], pool_actual, pool_max, pool_ignored)
         T = unit.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        acc_pool = self.empty((Pp,), torch.int32)
-        bin_of = self.empty((Pp,), torch.int32)
-        unacc = ctypes.c_int64(0)
-        evals = ctypes.c_uint64(0)
-        sel, keep_s = (None, None) if pod_class is None else \
-            self._selectors(classes, pod_class=pod_class, pool_match_ordered=pool_match)
-        aa, keep_a = (None, None) if pod_carries is None else self._anti_affinity(pod_carries, pod_matches_aa)
+        out, outs = self._fulfill_out(Pp, T)
+        sel, keep_s = self._selectors_if(classes, pod_class, pool_match_ordered=pool_match)
+        aa, keep_a = self._anti_affinity_if(pod_carries, pod_matches_aa)
         keep_p = [pod_requires, pod_self, pod_matches]
         pa = _native.PodAffinity(*[None if a is None else _ptr(a).value for a in keep_p], None)
         self._check(self._lib.acsfit_fulfill_pending_pa(
             self._ctx, _ptr(req), Pp, int(num_listed), D, _ptr(unit), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision),
-            None if sel is None else ctypes.cast(ctypes.byref(sel), ctypes.c_void_p),
-            None if aa is None else ctypes.cast(ctypes.byref(aa), ctypes.c_void_p),
-            ctypes.cast(ctypes.byref(pa), ctypes.c_void_p), int(present) & 0xFFFFFFFFFFFFFFFF, _ptr(new_size),
-            _ptr(units_needed), _ptr(bins_opened), _ptr(acc_pool), _ptr(bin_of),
-            ctypes.cast(ctypes.byref(unacc), ctypes.c_void_p), ctypes.cast(ctypes.byref(evals), ctypes.c_void_p),
-            self._stream()))
-        return {"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                "acc_pool": acc_pool, "bin_of": bin_of, "num_unaccounted": int(unacc.value),
-                "evals": int(evals.value)}
+            _ptr(pool_ignored), T, int(over_provision), _ref(sel), _ref(aa), _ref(pa),
+            int(present) & 0xFFFFFFFFFFFFFFFF, *outs, self._stream()))
+        return _fulfill_result(out)
 
     # ------------------------------------------------------------------ host-buffer entry points
     def scale_up_host(self, req, unit_all, unit_ordered, pool_actual, pool_max, pool_ignored, over_provision,
@@ -702,29 +622,14 @@ class Engine(object):
         node_type = _np(node_type, np.int32)
         assert isinstance(used, np.ndarray) and used.dtype == np.float64 and used.flags.c_contiguous
         N = used.shape[0]
-        unit_all = _np(unit_all, np.float64).reshape(-1, D)
-        unit_ordered = _np(unit_ordered, np.float64).reshape(-1, D)
+        unit_all, unit_ordered, pool_actual, pool_max, pool_ignored = _pools(D, [unit_all, unit_ordered], pool_actual,
+                                                                             pool_max, pool_ignored)
         T = unit_all.shape[0]
-        pool_actual = _np(pool_actual, np.int32)
-        pool_max = _np(pool_max, np.int32)
-        pool_ignored = _np(pool_ignored, np.uint8)
-        if out is None:
-            out = {"feasible": np.empty(P, dtype=np.uint8), "placed": np.empty(P, dtype=np.int32),
-                   "acc_pool": np.empty(P, dtype=np.int32)}
-        new_size = np.zeros(T, dtype=np.int64)
-        units_needed = np.zeros(T, dtype=np.int64)
-        bins_opened = np.zeros(T, dtype=np.int64)
-        counters = np.zeros(4, dtype=np.uint64)
+        res, outs, counters = _scale_up_out(_host_pod_outputs(P) if out is None else out, T)
         self._check(self._lib.acsfit_scale_up_host(
             self._ctx, _ptr(req), P, D, _ptr(unit_all), _ptr(unit_ordered), _ptr(pool_actual), _ptr(pool_max),
-            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), K, _ptr(node_type), _ptr(used), N,
-            _ptr(out["feasible"]), _ptr(out["placed"]), _ptr(new_size), _ptr(units_needed), _ptr(bins_opened),
-            _ptr(out["acc_pool"]), _ptr(counters)))
-        res = dict(out)
-        res.update({"new_size": new_size, "units_needed": units_needed, "bins_opened": bins_opened,
-                    "n_to_schedule": int(counters[0]), "n_pending": int(counters[1]),
-                    "num_unaccounted": int(counters[2]), "decisions": int(counters[3])})
-        return res
+            _ptr(pool_ignored), T, int(over_provision), _ptr(cap_type), K, _ptr(node_type), _ptr(used), N, *outs))
+        return _scale_up_result(res, counters)
 
     def occupancy_host(self, row_ptr, run_idx, req_run, used):
         """cluster.py:165-168 with HOST arrays; `used` [N, D] float64 is updated in place."""
