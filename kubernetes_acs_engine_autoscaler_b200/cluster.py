@@ -20,7 +20,7 @@ from . import utils
 from .deployments import Deployments
 from .engine_scaler import EngineScaler
 from .kube import KubeNode, KubePod, KubePodStatus
-from .scaler import LOG_DETAIL_LIMIT
+from .scaler import LOG_DETAIL_LIMIT, RULE_SWITCHES
 
 logger = logging.getLogger('autoscaler.cluster')
 
@@ -58,78 +58,17 @@ class Cluster(object):
                  node_taints=None, pod_anti_affinity=None, node_affinity=None, anti_affinity_node_states=None,
                  pod_affinity=None, pod_affinity_node_states=None, topology_spread=None,
                  topology_spread_node_states=None):
+        switches = locals()  # the rule switches as given, by name
         self.kubeconfig = kubeconfig
-        # honour the pods' spec.nodeSelector in the scale-up decision (opt-in; None: $ACSFIT_NODE_SELECTORS, off
-        # by default).  The reference ignores selectors, and the recorded reference ticks pin that behaviour.
-        if node_selectors is None:
-            node_selectors = os.environ.get('ACSFIT_NODE_SELECTORS', '0') not in ('', '0')
-        self.node_selectors = bool(node_selectors)
-        # with node selectors on, also in maintain: a node is pod-pending only when a pod to schedule matches it, so a
-        # pod pinned to one pool does not freeze scale-down in the others (opt-in; None: $ACSFIT_SELECTOR_NODE_STATES)
-        if selector_node_states is None:
-            selector_node_states = os.environ.get('ACSFIT_SELECTOR_NODE_STATES', '0') not in ('', '0')
-        elif selector_node_states and not self.node_selectors:
-            raise ValueError("selector_node_states=True needs node_selectors on")
-        self.selector_node_states = bool(selector_node_states) and self.node_selectors
-        # with node selectors on, a pod matches a node or pool only when it also tolerates every blocking taint there,
-        # so a tainted (e.g. GPU) pool neither absorbs nor holds back the pods it would refuse (opt-in; None:
-        # $ACSFIT_NODE_TAINTS)
-        if node_taints is None:
-            node_taints = os.environ.get('ACSFIT_NODE_TAINTS', '0') not in ('', '0')
-        elif node_taints and not self.node_selectors:
-            raise ValueError("node_taints=True needs node_selectors on")
-        self.node_taints = bool(node_taints) and self.node_selectors
-        # with node selectors on, a pod matches a node or pool only when its required node affinity admits it too, so a
-        # pod pinned to a pool by affinity neither "fits" other pools' nodes nor holds them back (opt-in; None:
-        # $ACSFIT_NODE_AFFINITY)
-        if node_affinity is None:
-            node_affinity = os.environ.get('ACSFIT_NODE_AFFINITY', '0') not in ('', '0')
-        elif node_affinity and not self.node_selectors:
-            raise ValueError("node_affinity=True needs node_selectors on")
-        self.node_affinity = bool(node_affinity) and self.node_selectors
-        # honour required pod anti-affinity with topologyKey kubernetes.io/hostname in first fit and bin packing, so that
-        # replicas which avoid each other are not simulated onto one node (opt-in; None: $ACSFIT_POD_ANTI_AFFINITY).
-        # Independent of node_selectors; with both on, the node pass uses both.
-        if pod_anti_affinity is None:
-            pod_anti_affinity = os.environ.get('ACSFIT_POD_ANTI_AFFINITY', '0') not in ('', '0')
-        self.pod_anti_affinity = bool(pod_anti_affinity)
-        # with pod anti-affinity on, also in maintain: a node is pod-pending only when some pod to schedule could land on
-        # it given the pods already there, so a pending replica does not freeze the nodes that run its siblings
-        # (opt-in; None: $ACSFIT_ANTI_AFFINITY_NODE_STATES).  With selector_node_states on, both rules apply.
-        if anti_affinity_node_states is None:
-            anti_affinity_node_states = os.environ.get('ACSFIT_ANTI_AFFINITY_NODE_STATES', '0') not in ('', '0')
-        elif anti_affinity_node_states and not self.pod_anti_affinity:
-            raise ValueError("anti_affinity_node_states=True needs pod_anti_affinity on")
-        self.anti_affinity_node_states = bool(anti_affinity_node_states) and self.pod_anti_affinity
-        # honour required pod affinity with topologyKey kubernetes.io/hostname in first fit and bin packing, so that a pod
-        # which must sit beside another is neither simulated onto a node without one nor packed into a new node alone
-        # (opt-in; None: $ACSFIT_POD_AFFINITY).  Independent of node selectors and anti-affinity.
-        if pod_affinity is None:
-            pod_affinity = os.environ.get('ACSFIT_POD_AFFINITY', '0') not in ('', '0')
-        self.pod_affinity = bool(pod_affinity)
-        # with pod affinity on, also in maintain: a node is pod-pending only when some pod to schedule could land on it
-        # given its required pod affinity, so a pod that needs a pod elsewhere does not freeze every idle node (opt-in;
-        # None: $ACSFIT_POD_AFFINITY_NODE_STATES).  Combines with selector_node_states and anti_affinity_node_states.
-        if pod_affinity_node_states is None:
-            pod_affinity_node_states = os.environ.get('ACSFIT_POD_AFFINITY_NODE_STATES', '0') not in ('', '0')
-        elif pod_affinity_node_states and not self.pod_affinity:
-            raise ValueError("pod_affinity_node_states=True needs pod_affinity on")
-        self.pod_affinity_node_states = bool(pod_affinity_node_states) and self.pod_affinity
+        # each rule switch: None reads its environment variable, and it is on only while its prerequisite is on
+        for name, env, needs in RULE_SWITCHES:
+            value = switches[name]
+            if value is None:
+                value = os.environ.get(env, '0') not in ('', '0')
+            elif value and needs and not getattr(self, needs):
+                raise ValueError("%s=True needs %s on" % (name, needs))
+            setattr(self, name, bool(value) and (needs is None or getattr(self, needs)))
         self.affinity_present = set()  # signatures the last node pass left on some node (scale() hands them on)
-        # honour topologySpreadConstraints with topologyKey kubernetes.io/hostname and whenUnsatisfiable DoNotSchedule in
-        # first fit and bin packing, so that replicas spread over nodes are not simulated onto one roomy node (opt-in;
-        # None: $ACSFIT_TOPOLOGY_SPREAD).  Independent of the other switches.
-        if topology_spread is None:
-            topology_spread = os.environ.get('ACSFIT_TOPOLOGY_SPREAD', '0') not in ('', '0')
-        self.topology_spread = bool(topology_spread)
-        # with topology spread on, also in maintain: a node is pod-pending only when some pod to schedule could land on it
-        # given its spread constraint, so a replica that may not stack beside its siblings does not freeze their nodes
-        # (opt-in; None: $ACSFIT_TOPOLOGY_SPREAD_NODE_STATES).  Combines with the other node-states switches.
-        if topology_spread_node_states is None:
-            topology_spread_node_states = os.environ.get('ACSFIT_TOPOLOGY_SPREAD_NODE_STATES', '0') not in ('', '0')
-        elif topology_spread_node_states and not self.topology_spread:
-            raise ValueError("topology_spread_node_states=True needs topology_spread on")
-        self.topology_spread_node_states = bool(topology_spread_node_states) and self.topology_spread
         self.other_nodes = []  # the listed nodes that are not agents (the master): domains of the spread constraints
         self.service_principal_app_id = service_principal_app_id
         self.service_principal_secret = service_principal_secret
@@ -233,12 +172,8 @@ class Cluster(object):
             resource_group=self.resource_group, nodes=all_nodes, deployments=self.deployments,
             arm_template=self.arm_template, arm_parameters=self.arm_parameters, dry_run=self.dry_run,
             ignore_pools=self.ignore_pools, over_provision=self.over_provision, spare_count=self.spare_agents,
-            idle_threshold=self.idle_threshold, notifier=self.notifier, node_selectors=self.node_selectors,
-            selector_node_states=self.selector_node_states, node_taints=self.node_taints,
-            pod_anti_affinity=self.pod_anti_affinity, node_affinity=self.node_affinity,
-            anti_affinity_node_states=self.anti_affinity_node_states, pod_affinity=self.pod_affinity,
-            pod_affinity_node_states=self.pod_affinity_node_states, topology_spread=self.topology_spread,
-            topology_spread_node_states=self.topology_spread_node_states, other_nodes=self.other_nodes)
+            idle_threshold=self.idle_threshold, notifier=self.notifier, other_nodes=self.other_nodes,
+            **{name: getattr(self, name) for name, _, _ in RULE_SWITCHES})
 
         pods = kube.make_pods(self.list_pods()) if KubePod is kube.KubePod else list(map(KubePod, self.list_pods()))
         running_or_pending_assigned_pods = [

@@ -12,31 +12,24 @@ from . import adapters
 from . import snapshot
 from . import utils
 from .agent_pool import AgentPool
-from .scaler import STATE_NAMES, ClusterNodeState, Scaler
+from .scaler import RULE_SWITCHES, STATE_NAMES, ClusterNodeState, Scaler
 
 logger = logging.getLogger('autoscaler.engine_scaler')
 
 ACT_NONE, ACT_CORDON_DRAIN, ACT_CORDON, ACT_UNCORDON, ACT_SCALE_IN = range(5)
+SWITCH_NAMES = frozenset(name for name, _, _ in RULE_SWITCHES)
 
 
 class EngineScaler(Scaler):
     def __init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
-                 deployments, arm_template, arm_parameters, ignore_pools, notifier, node_selectors=False,
-                 selector_node_states=False, node_taints=False, pod_anti_affinity=False, node_affinity=False,
-                 anti_affinity_node_states=False, pod_affinity=False, pod_affinity_node_states=False,
-                 topology_spread=False, topology_spread_node_states=False, other_nodes=()):
+                 deployments, arm_template, arm_parameters, ignore_pools, notifier, *, other_nodes=(), **switches):
+        """`switches`: the rule switches of scaler.RULE_SWITCHES by name (False when not given)"""
         Scaler.__init__(self, resource_group, nodes, over_provision, spare_count, idle_threshold, dry_run,
                         deployments, notifier)
-        self.node_selectors = node_selectors
-        self.selector_node_states = selector_node_states
-        self.node_taints = node_taints
-        self.node_affinity = node_affinity
-        self.pod_anti_affinity = pod_anti_affinity
-        self.anti_affinity_node_states = anti_affinity_node_states
-        self.pod_affinity = pod_affinity
-        self.pod_affinity_node_states = pod_affinity_node_states
-        self.topology_spread = topology_spread
-        self.topology_spread_node_states = topology_spread_node_states
+        for name, value in switches.items():
+            if name not in SWITCH_NAMES:
+                raise TypeError("EngineScaler() got an unexpected keyword argument '%s'" % name)
+            setattr(self, name, value)
         self.other_nodes = list(other_nodes)
         self.arm_parameters = arm_parameters
         self.arm_template = arm_template

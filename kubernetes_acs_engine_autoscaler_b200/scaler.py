@@ -37,6 +37,31 @@ STATE_NAMES = [
 # per-pod log lines are only emitted up to this many pods (SURVEY.md section 5: O(P) strings)
 LOG_DETAIL_LIMIT = 20000
 
+# The opt-in scheduling rules, all off by default: (switch, environment variable read when Cluster gets None, the switch
+# it needs on or None).  Cluster resolves them in this order and hands them to EngineScaler by name.
+RULE_SWITCHES = (
+    # honour spec.nodeSelector in scale-up; the reference ignores selectors, and its recorded ticks pin that
+    ('node_selectors', 'ACSFIT_NODE_SELECTORS', None),
+    # in maintain too: a pod pinned to one pool does not freeze scale-down in the others
+    ('selector_node_states', 'ACSFIT_SELECTOR_NODE_STATES', 'node_selectors'),
+    # a tainted (e.g. GPU) pool neither absorbs nor holds back the pods that do not tolerate its taints
+    ('node_taints', 'ACSFIT_NODE_TAINTS', 'node_selectors'),
+    # a pod pinned to a pool by required node affinity neither fits nor holds back other pools' nodes
+    ('node_affinity', 'ACSFIT_NODE_AFFINITY', 'node_selectors'),
+    # replicas that avoid each other (hostname anti-affinity) are not simulated onto one node or new node
+    ('pod_anti_affinity', 'ACSFIT_POD_ANTI_AFFINITY', None),
+    # in maintain too: a pending replica does not freeze the nodes that run its siblings
+    ('anti_affinity_node_states', 'ACSFIT_ANTI_AFFINITY_NODE_STATES', 'pod_anti_affinity'),
+    # a pod that must sit beside another (hostname affinity) lands neither on a node without one nor alone
+    ('pod_affinity', 'ACSFIT_POD_AFFINITY', None),
+    # in maintain too: a pod that needs a pod elsewhere does not freeze every idle node
+    ('pod_affinity_node_states', 'ACSFIT_POD_AFFINITY_NODE_STATES', 'pod_affinity'),
+    # replicas spread over hostnames (DoNotSchedule) are not simulated onto one roomy node
+    ('topology_spread', 'ACSFIT_TOPOLOGY_SPREAD', None),
+    # in maintain too: a replica that may not stack beside its siblings does not freeze their nodes
+    ('topology_spread_node_states', 'ACSFIT_TOPOLOGY_SPREAD_NODE_STATES', 'topology_spread'),
+)
+
 
 class Scaler(object):
     # a node is under-utilised when its busy pods use <= 30 % of every capacity dimension
@@ -61,30 +86,8 @@ class Scaler(object):
         self.agent_pools = None
         self.scalable_pools = None
         self.ignored_pool_names = {}
-        self.node_selectors = False  # honour the pods' nodeSelectors (Cluster(node_selectors=...))
-        # POD_PENDING only when a pod to schedule matches the node (Cluster(selector_node_states=...))
-        self.selector_node_states = False
-        # with node selectors: a pod matches a node or pool only when it also tolerates its blocking taints
-        # (Cluster(node_taints=...))
-        self.node_taints = False
-        # with node selectors: a pod matches a node or pool only when its required node affinity admits it too
-        # (Cluster(node_affinity=...))
-        self.node_affinity = False
-        # required pod anti-affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_anti_affinity=...))
-        self.pod_anti_affinity = False
-        # with pod anti-affinity: POD_PENDING only when some pod to schedule could land on the node given the pods
-        # already there (Cluster(anti_affinity_node_states=...))
-        self.anti_affinity_node_states = False
-        # required pod affinity (hostname topology) in the bins of fulfill_pending (Cluster(pod_affinity=...))
-        self.pod_affinity = False
-        # with pod affinity: POD_PENDING only when some pod to schedule could land on the node given its required pod
-        # affinity (Cluster(pod_affinity_node_states=...))
-        self.pod_affinity_node_states = False
-        # hostname topology spread (DoNotSchedule) in the bins of fulfill_pending (Cluster(topology_spread=...))
-        self.topology_spread = False
-        # with topology spread: POD_PENDING only when some pod to schedule could land on the node given its spread
-        # constraint (Cluster(topology_spread_node_states=...))
-        self.topology_spread_node_states = False
+        for name, _, _ in RULE_SWITCHES:  # Cluster(<name>=...)
+            setattr(self, name, False)
         # the listed nodes that are not agents (the master): domains of the spread constraints
         self.other_nodes = []
 

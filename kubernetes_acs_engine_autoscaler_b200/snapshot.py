@@ -123,6 +123,16 @@ def _node_types(nodes, dims):
     return cap, node_type
 
 
+def _dev_masks(eng, *masks):
+    """uint64 mask arrays -> int64 device tensors (the Engine takes masks as int64)"""
+    return tuple(eng.dev(a.view(np.int64), torch.int64) for a in masks)
+
+
+def _live(rule):
+    """the rule when it can constrain a pod of the call, else None (the Engine forms without it give the same result)"""
+    return rule if rule is not None and not rule.trivial else None
+
+
 def _write_back_used(nodes, dims, used, touched_keys):
     """store used[n] into node.used_capacity with the key set the reference would hold: the
     node's previous keys plus the keys of every pod counted on it (KubeResource.__add__ unions)."""
@@ -156,6 +166,12 @@ class SelectorClasses(object):
     def trivial(self):
         """every pod is class 0 (no selector, or one that matches every node and pool)"""
         return not self.pod_class.any()
+
+    def to_device(self, eng, nodes=True):
+        """the Engine's selector arguments: (pod_class, node_match, classes) of a node pass, node_match on the device,
+        or with nodes=False (pod_class, pool_match, classes) of a bin pass, pool_match on the host"""
+        return (eng.dev(self.pod_class, torch.uint8), _dev_masks(eng, self.node_match)[0] if nodes else self.pool_match,
+                self.classes)
 
 
 def _selector_matches(labels, items):
@@ -395,6 +411,12 @@ class AntiAffinity(object):
         """no term can block a pod of this call: the plain entry points give the same result"""
         return not self.terms
 
+    def to_device(self, eng, nodes=True):
+        """the Engine's anti-affinity arguments on the device: pod_carries, pod_matches and, with `nodes`,
+        node_carries and node_matches"""
+        masks = (self.pod_carries, self.pod_matches) + ((self.node_carries, self.node_matches) if nodes else ())
+        return _dev_masks(eng, *masks)
+
 
 def _pod_projection(pods, keys):
     """(group[len(pods)], proj[G, 1 + len(keys)], code_of): the pods grouped by (namespace, the values of the label keys
@@ -576,6 +598,11 @@ class PodAffinity(object):
         """no pod of this call has a signature: the calls without pod affinity give the same result"""
         return not self.signatures
 
+    def to_device(self, eng, nodes=True):
+        """the Engine's pod-affinity arguments on the device: pod_requires, pod_self, pod_matches and, with `nodes`,
+        node_has"""
+        return _dev_masks(eng, self.pod_requires, self.pod_self, self.pod_matches, *((self.node_has,) if nodes else ()))
+
 
 def pod_affinity(pods, nodes=(), running_pods=()):
     """signature masks of the pods to place (`pods`) and of the nodes (the pods of `running_pods` on them count, matched
@@ -683,6 +710,15 @@ class TopologySpread(object):
     def trivial(self):
         """no pod of this call has a constraint: the calls without topology spread give the same result"""
         return not self.keys
+
+    def to_device(self, eng, nodes=True):
+        """the Engine's topology-spread arguments: the key count, pod_key, pod_skew and pod_matches on the device and,
+        with `nodes`, node_count and node_domain on the device and floor on the host"""
+        pods = (len(self.keys), eng.dev(self.pod_key, torch.uint8), eng.dev(self.pod_skew, torch.int32),
+                *_dev_masks(eng, self.pod_matches))
+        if not nodes:
+            return pods
+        return pods + (eng.dev(self.node_count, torch.int32), *_dev_masks(eng, self.node_domain), self.floor)
 
 
 def _spread_domains(pods, constraints, all_nodes):
@@ -805,9 +841,9 @@ def feasible_pods(pods, agent_pools, classes=None):
     bad = _nonfinite_rows(req)       # an infinite request fits nowhere (cap - inf < 0)
     req[bad] = 0.0
     eng = get_engine()
-    if classes is not None and not classes.trivial:
+    if _live(classes) is not None:
         mask, _ = eng.feasible_mask_sel(eng.dev(req, torch.float64), eng.dev(unit, torch.float64),
-                                        eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
+                                        *classes.to_device(eng, nodes=False))
     else:
         mask, _ = eng.feasible_mask(eng.dev(req, torch.float64), eng.dev(unit, torch.float64))
     out = mask.cpu().numpy().astype(bool)
@@ -877,94 +913,39 @@ def first_fit_nodes(pods, nodes, classes=None, anti_affinity=None, pod_affinity=
     used = dims.rows(n.used_capacity for n in nodes)
     req[bad] = 0.0
     eng = get_engine()
+    sel, aa, pa, ts = map(_live, (classes, anti_affinity, pod_affinity, topology_spread))
+    d_sel, d_aa, d_pa, d_ts = (None if r is None else r.to_device(eng) for r in (sel, aa, pa, ts))
     d_used = eng.dev(used, torch.float64)
-    sel = classes is not None and not classes.trivial
-    if topology_spread is not None and not topology_spread.trivial:
-        ts = topology_spread
-        pa = pod_affinity if pod_affinity is not None and not pod_affinity.trivial else None
-        aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
-        d_nh = d_nc = d_nx = None
-        pa_args = aa_args = None
-        if pa is not None:
-            d_nh = eng.dev(pa.node_has.view(np.int64), torch.int64)
-            pa_args = tuple(eng.dev(a.view(np.int64), torch.int64) for a in (pa.pod_requires, pa.pod_self,
-                                                                               pa.pod_matches)) + (d_nh,)
-        if aa is not None:
-            d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
-            aa_args = (eng.dev(aa.pod_carries.view(np.int64), torch.int64),
-                       eng.dev(aa.pod_matches.view(np.int64), torch.int64), d_nc, d_nx)
-        d_cnt = eng.dev(np.ascontiguousarray(ts.node_count), torch.int32)
-        d_placed, _ = eng.first_fit_nodes_ts(eng.dev(req, torch.float64),
-                                             None if not bad.any() else eng.dev(ok_idx, torch.int32),
-                                             eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
-                                             len(ts.keys), eng.dev(ts.pod_key, torch.uint8),
-                                             eng.dev(ts.pod_skew, torch.int32),
-                                             eng.dev(ts.pod_matches.view(np.int64), torch.int64), d_cnt,
-                                             eng.dev(ts.node_domain.view(np.int64), torch.int64), ts.floor,
-                                             pa=pa_args, aa=aa_args,
-                                             **(dict(pod_class=eng.dev(classes.pod_class, torch.uint8),
-                                                     node_match=eng.dev(classes.node_match.view(np.int64), torch.int64),
-                                                     classes=classes.classes) if sel else {}))
-        ts.node_count[:] = d_cnt.cpu().numpy()
-        if pa is not None:
-            pa.node_has[:] = d_nh.cpu().numpy().view(np.uint64)
-        if aa is not None:
-            aa.node_carries[:] = d_nc.cpu().numpy().view(np.uint64)
-            aa.node_matches[:] = d_nx.cpu().numpy().view(np.uint64)
-    elif pod_affinity is not None and not pod_affinity.trivial:
-        pa = pod_affinity
-        aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
-        d_nh = eng.dev(pa.node_has.view(np.int64), torch.int64)
-        d_nc = d_nx = None
-        aa_args = ()
-        if aa is not None:
-            d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
-            aa_args = (eng.dev(aa.pod_carries.view(np.int64), torch.int64),
-                       eng.dev(aa.pod_matches.view(np.int64), torch.int64), d_nc, d_nx)
-        d_placed, _ = eng.first_fit_nodes_pa(eng.dev(req, torch.float64),
-                                             None if not bad.any() else eng.dev(ok_idx, torch.int32),
-                                             eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
-                                             eng.dev(pa.pod_requires.view(np.int64), torch.int64),
-                                             eng.dev(pa.pod_self.view(np.int64), torch.int64),
-                                             eng.dev(pa.pod_matches.view(np.int64), torch.int64), d_nh, *aa_args,
-                                             **(dict(pod_class=eng.dev(classes.pod_class, torch.uint8),
-                                                     node_match=eng.dev(classes.node_match.view(np.int64), torch.int64),
-                                                     classes=classes.classes) if sel else {}))
-        pa.node_has[:] = d_nh.cpu().numpy().view(np.uint64)
-        if aa is not None:
-            aa.node_carries[:] = d_nc.cpu().numpy().view(np.uint64)
-            aa.node_matches[:] = d_nx.cpu().numpy().view(np.uint64)
-    elif anti_affinity is not None and not anti_affinity.trivial:
-        aa = anti_affinity
-        d_nc, d_nx = eng.dev(aa.node_carries.view(np.int64), torch.int64), eng.dev(aa.node_matches.view(np.int64), torch.int64)
-        d_placed, _ = eng.first_fit_nodes_aa(eng.dev(req, torch.float64),
-                                             None if not bad.any() else eng.dev(ok_idx, torch.int32),
-                                             eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
-                                             eng.dev(aa.pod_carries.view(np.int64), torch.int64),
-                                             eng.dev(aa.pod_matches.view(np.int64), torch.int64), d_nc, d_nx,
-                                             *((eng.dev(classes.pod_class, torch.uint8),
-                                                eng.dev(classes.node_match.view(np.int64), torch.int64),
-                                                classes.classes) if sel else ()))
-        aa.node_carries[:] = d_nc.cpu().numpy().view(np.uint64)
-        aa.node_matches[:] = d_nx.cpu().numpy().view(np.uint64)
-    elif sel:
-        d_placed, _ = eng.first_fit_nodes_sel(eng.dev(req, torch.float64),
-                                              None if not bad.any() else eng.dev(ok_idx, torch.int32),
-                                              eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used,
-                                              eng.dev(classes.pod_class, torch.uint8),
-                                              eng.dev(classes.node_match.view(np.int64), torch.int64), classes.classes)
+    head = (eng.dev(req, torch.float64), None if not bad.any() else eng.dev(ok_idx, torch.int32),
+            eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used)
+    sel_kw = {} if sel is None else dict(zip(("pod_class", "node_match", "classes"), d_sel))
+    if ts is not None:
+        d_placed, _ = eng.first_fit_nodes_ts(*head, *d_ts, pa=d_pa, aa=d_aa, **sel_kw)
+    elif pa is not None:
+        d_placed, _ = eng.first_fit_nodes_pa(*head, *d_pa, *(d_aa or ()), **sel_kw)
+    elif aa is not None:
+        d_placed, _ = eng.first_fit_nodes_aa(*head, *d_aa, *(d_sel or ()))
+    elif sel is not None:
+        d_placed, _ = eng.first_fit_nodes_sel(*head, *d_sel)
     else:
-        d_placed, _ = eng.first_fit_nodes(eng.dev(req, torch.float64),
-                                          None if not bad.any() else eng.dev(ok_idx, torch.int32),
-                                          eng.dev(cap, torch.float64), eng.dev(node_type, torch.int32), d_used)
+        d_placed, _ = eng.first_fit_nodes(*head)
+    updated = []  # (host array, device tensor) of the rules' node arrays the call updated in place
+    if ts is not None:
+        updated.append((ts.node_count, d_ts[4]))
+    if pa is not None:
+        updated.append((pa.node_has, d_pa[3]))
+    if aa is not None:
+        updated += [(aa.node_carries, d_aa[2]), (aa.node_matches, d_aa[3])]
+    for host, d in updated:
+        host[...] = d.cpu().numpy().view(host.dtype)
     res = d_placed.cpu().numpy()
     if bad.any():
         placed[ok_idx] = res
     else:
         placed = res
     used = d_used.cpu().numpy()
-    sel = np.nonzero(placed >= 0)[0]
-    _write_back_used(nodes, dims, used, _touched_keys(placed[sel], inv_req[sel], uniq_req))
+    took = np.nonzero(placed >= 0)[0]
+    _write_back_used(nodes, dims, used, _touched_keys(placed[took], inv_req[took], uniq_req))
     return placed
 
 
@@ -1009,45 +990,21 @@ def fulfill(unique_pods, num_listed, ordered_pools, ignored_pool_names, over_pro
     pools = (np.asarray([pool.actual_capacity for pool in ordered_pools], dtype=np.int32),
              np.asarray([min(pool.max_size, 2 ** 31 - 1) for pool in ordered_pools], dtype=np.int32),
              np.asarray([1 if pool.name in ignored_pool_names else 0 for pool in ordered_pools], dtype=np.uint8))
-    sel = classes is not None and not classes.trivial
-    if topology_spread is not None and not topology_spread.trivial:
-        ts = topology_spread
-        pa = pod_affinity if pod_affinity is not None and not pod_affinity.trivial else None
-        aa = anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
-        present = 0 if pa is None else sum(1 << k for k, sig in enumerate(pa.signatures) if sig in affinity_present)
-        res = eng.fulfill_pending_ts(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
-                                     len(ts.keys), eng.dev(ts.pod_key, torch.uint8), eng.dev(ts.pod_skew, torch.int32),
-                                     eng.dev(ts.pod_matches.view(np.int64), torch.int64),
-                                     pa=None if pa is None else tuple(eng.dev(a.view(np.int64), torch.int64) for a in (
-                                         pa.pod_requires, pa.pod_self, pa.pod_matches)),
-                                     present=present,
-                                     aa=None if aa is None else (eng.dev(aa.pod_carries.view(np.int64), torch.int64),
-                                                                 eng.dev(aa.pod_matches.view(np.int64), torch.int64)),
-                                     **(dict(pod_class=eng.dev(classes.pod_class, torch.uint8),
-                                             pool_match=classes.pool_match, classes=classes.classes) if sel else {}))
-    elif pod_affinity is not None and not pod_affinity.trivial:
-        pa, aa = pod_affinity, anti_affinity if anti_affinity is not None and not anti_affinity.trivial else None
-        present = sum(1 << k for k, sig in enumerate(pa.signatures) if sig in affinity_present)
-        res = eng.fulfill_pending_pa(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
-                                     eng.dev(pa.pod_requires.view(np.int64), torch.int64),
-                                     eng.dev(pa.pod_self.view(np.int64), torch.int64),
-                                     eng.dev(pa.pod_matches.view(np.int64), torch.int64), present,
-                                     *((eng.dev(aa.pod_carries.view(np.int64), torch.int64),
-                                        eng.dev(aa.pod_matches.view(np.int64), torch.int64)) if aa is not None else
-                                       (None, None)),
-                                     *((eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
-                                       if sel else ()))
-    elif anti_affinity is not None and not anti_affinity.trivial:
-        res = eng.fulfill_pending_aa(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
-                                     eng.dev(anti_affinity.pod_carries.view(np.int64), torch.int64),
-                                     eng.dev(anti_affinity.pod_matches.view(np.int64), torch.int64),
-                                     *((eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
-                                       if sel else ()))
-    elif sel:
-        res = eng.fulfill_pending_sel(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision,
-                                      eng.dev(classes.pod_class, torch.uint8), classes.pool_match, classes.classes)
+    sel, aa, pa, ts = map(_live, (classes, anti_affinity, pod_affinity, topology_spread))
+    d_sel, d_aa, d_pa, d_ts = (None if r is None else r.to_device(eng, nodes=False) for r in (sel, aa, pa, ts))
+    present = 0 if pa is None else sum(1 << k for k, sig in enumerate(pa.signatures) if sig in affinity_present)
+    head = (eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision)
+    sel_kw = {} if sel is None else dict(zip(("pod_class", "pool_match", "classes"), d_sel))
+    if ts is not None:
+        res = eng.fulfill_pending_ts(*head, *d_ts, pa=d_pa, present=present, aa=d_aa, **sel_kw)
+    elif pa is not None:
+        res = eng.fulfill_pending_pa(*head, *d_pa, present, *(d_aa or (None, None)), *(d_sel or ()))
+    elif aa is not None:
+        res = eng.fulfill_pending_aa(*head, *d_aa, *(d_sel or ()))
+    elif sel is not None:
+        res = eng.fulfill_pending_sel(*head, *d_sel)
     else:
-        res = eng.fulfill_pending(eng.dev(req, torch.float64), num_listed, unit, *pools, over_provision)
+        res = eng.fulfill_pending(*head)
     res["acc_pool"] = res["acc_pool"].cpu().numpy()
     res["bin_of"] = res["bin_of"].cpu().numpy()
     return res
@@ -1215,21 +1172,17 @@ def node_states(nodes, pods_lists, any_pending, idle_threshold, no_match=None, a
         rows = admit.row_carries if admit.row_carries is not None else admit.row_has
         if rows is not None and len(rows) != len(flat):
             raise ValueError("pending_admit masks of %d pods for a table of %d" % (len(rows), len(flat)))
-        dev_masks = lambda a: None if a is None else eng.dev(a.view(np.int64), torch.int64)  # noqa: E731
-        if admit.sig_key is not None:
-            eng.pending_admit_ts(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
-                                 dev_masks(admit.row_has), dev_masks(admit.node_match), admit.sig_class,
-                                 admit.sig_carries, admit.sig_matches, admit.sig_need, admit.sig_key, admit.sig_skew,
-                                 admit.node_count.shape[0], eng.dev(admit.node_count, torch.int32),
-                                 dev_masks(admit.node_domain), admit.floor, d_node_flags)
-        elif admit.row_has is None:
-            eng.pending_admit(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
-                              dev_masks(admit.node_match), admit.sig_class, admit.sig_carries, admit.sig_matches,
-                              d_node_flags)
-        else:
-            eng.pending_admit_pa(d_row_ptr, dev_masks(admit.row_carries), dev_masks(admit.row_matches),
-                                 dev_masks(admit.row_has), dev_masks(admit.node_match), admit.sig_class,
-                                 admit.sig_carries, admit.sig_matches, admit.sig_need, d_node_flags)
+        dev_masks = lambda a: None if a is None else _dev_masks(eng, a)[0]  # noqa: E731
+        ts = admit.sig_key is not None
+        pa = ts or admit.row_has is not None  # the _pa and _ts forms take the pod-affinity arrays, None or not
+        rows = [dev_masks(admit.row_carries), dev_masks(admit.row_matches)] + \
+            ([dev_masks(admit.row_has)] if pa else [])
+        sigs = [admit.sig_class, admit.sig_carries, admit.sig_matches] + ([admit.sig_need] if pa else [])
+        if ts:
+            sigs += [admit.sig_key, admit.sig_skew, admit.node_count.shape[0], eng.dev(admit.node_count, torch.int32),
+                     dev_masks(admit.node_domain), admit.floor]
+        admit_fn = eng.pending_admit_ts if ts else eng.pending_admit_pa if pa else eng.pending_admit
+        admit_fn(d_row_ptr, *rows, dev_masks(admit.node_match), *sigs, d_node_flags)
     st = eng.node_states(d_row_ptr,
                          None,  # contiguous table: the rows ARE in node order (bulk-copy streaming kernel)
                          eng.dev(req_run, torch.float64), eng.dev(flags, torch.uint8),
